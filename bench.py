@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- benchmark of the B200-native Kaiju classification path.
+"""bench.py -- benchmark of the H100-native Kaiju classification path.
 
 Metric (BASELINE.json): read items/s (one item = one output line; a pair counts once) for 150 bp paired reads, MEM mode
--m 11 (default SEG on), against a viruses-scale .fmi, at N = 1/2/4/8 B200 -- next to the reference CPU `kaiju -z <best>`.
+-m 11 (default SEG on), against a viruses-scale .fmi, at N = 1/2/4/8 H100 -- next to the reference CPU `kaiju -z <best>`.
 
 Headline workload (configs[1]): 10 M synthetic PE150 pairs per GPU per step (SURVEY.md 8d recipe, tools/kjgen.c, seeded) against the
 "synth-viruses" stand-in (680 k proteins, ~2e8 letters; the real kaiju_db_viruses.fmi needs a download), whose .fmi is built here with
@@ -16,10 +16,14 @@ the reference's own kaiju-mkbwt/kaiju-mkfmi (-e 3).  A "step" is one pass of the
                best point reported; its output on the sample is compared read by read with the GPU's (`parity`)
   configs    : (N = 1 only) the other BASELINE.json configurations in the same run, each with value / e2e / roofline / cpu_baseline / parity:
                greedy      = configs[2]: `-a greedy -e 3 -s 65` on the same 10 M pairs
-               large_index = configs[3]: MEM on a refseq_ref-scale index (2.7e10 BWT rows, ~126 GB in HBM): the index of the collection
-                             in which every synth-viruses protein occurs K times, built on the device by kj_create_scaled (the
-                             reference's index builder cannot produce 2.7e10 rows inside a benchmark run; K-fold == what
+               large_index = configs[3]: MEM on a large index (1.2e10 BWT rows, ~57 GB in HBM: a round size that fits an 80 GB H100
+                             next to the base index and the reads; a refseq_ref-scale index of 2.7e10 rows does not): the index of the
+                             collection in which every synth-viruses protein occurs K times, built on the device by kj_create_scaled (the
+                             reference's index builder cannot produce 1.2e10 rows inside a benchmark run; K-fold == what
                              kaiju-mkbwt builds for the K-fold FASTA, tests/test_gpu_build.py); results must equal the base index's
+
+Every timed loop (value, e2e, strong_scaling, configs) runs exactly --steps steps.  --dump-outputs DIR writes what the headline path
+(kj_classify_device2) returned in its last timed step, for a fixed seeded sample of the reads, as DIR/<name>.npy (see dump_outputs()).
 
 Multi-GPU: one process per GPU (torchrun), index replicated, reads sharded (weak scaling), ONE NCCL all-gather of the per-read dense
 taxon indices (uint32) per step on a side stream, overlapped with the next step; `strong_scaling` = the 10 M-pair job split over N.
@@ -46,7 +50,8 @@ def parse():
     ap.add_argument("--workdir", default=os.environ.get("KJ_BENCH_DIR", "/tmp/kjbench"))
     ap.add_argument("--skip-cpu", action="store_true", help="no CPU legs (roofline numerator, cpu_baseline, parity)")
     ap.add_argument("--headline-only", action="store_true", help="skip the `configs` sub-runs (greedy, large_index)")
-    ap.add_argument("--large-rows", type=float, default=2.7e10, help="target BWT rows of the large_index config (0 = skip)")
+    ap.add_argument("--large-rows", type=float, default=1.2e10, help="target BWT rows of the large_index config (0 = skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the headline path's outputs of its last timed step to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -91,7 +96,16 @@ class ClockSampler(threading.Thread):
             if any(len(r) > col and r[col].lower().startswith("active") for r in self.rows):
                 reasons.append(name)
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": int(float(self.rows[0][1])) if self.rows[0][1].replace(".", "").isdigit() else None,
-                "reasons": reasons, "samples": len(self.rows)}
+                "reasons": reasons, "samples": len(self.rows), "gpu": self.card()}
+
+    def card(self):
+        """Name and power limit of the card the numbers were measured on (part of every absolute number)."""
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                                 stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=5).stdout.decode().strip().split(",")
+            return {"name": out[0].strip(), "power_limit_w": float(out[1])}
+        except Exception:
+            return None
 
 
 # ---------------------------------------------------------------------------------------------------- reference CPU legs
@@ -194,7 +208,7 @@ def reference_arm(args):
     emit(line)
 
 
-# ---------------------------------------------------------------------------------------------------- B200 arm
+# ---------------------------------------------------------------------------------------------------- GPU arm
 class Runner:
     """Reads of one rank (pinned host + device copies) and the timed loops over one Classifier."""
 
@@ -277,18 +291,41 @@ class Runner:
         return float(t.item()), clf.kernel_launches - l0
 
 
-def measure(R, clf, steps, warmup, world):
-    """value (device-resident) and e2e (host buffers) of one configuration on runner R."""
+def measure(R, clf, steps, warmup, world, keep_outputs=False):
+    """value (device-resident) and e2e (host buffers) of one configuration on runner R; keep_outputs: also return (under "outputs") what the
+    device-resident path returned in its last timed step, copied before the e2e loop overwrites the dense-index buffers."""
     ms_dev, launches = R.timed(clf, R.step_device, steps, max(3, warmup))
     kernel_ms = clf.last_kernel_ms                                   # CUDA events around the last classify kernel, on its launch stream
-    e2e_steps = max(2, steps // 2)
-    ms_host, _ = R.timed(clf, R.step_host, e2e_steps, 1)
+    outputs = None
+    if keep_outputs:
+        outputs = {"taxon": R.d_tax.cpu().numpy().view(np.uint64), "best": R.d_best.cpu().numpy().view(np.uint32),
+                   "taxon_index": R.d_compact[(R.i - 1) & 1].cpu().numpy().view(np.uint32)}
+    ms_host, _ = R.timed(clf, R.step_host, steps, 1)
     clf.check_errors()
     assert R.torch.equal(R.h_tax, R.d_tax.cpu()), "host-buffer and device-buffer entry points disagree"
     total = R.n * world
-    return {"value": total * steps / (ms_dev / 1000.0), "ms_per_step": ms_dev / steps, "kernel_ms": kernel_ms, "gpu_launches": int(launches),
-            "e2e": {"value": total * e2e_steps / (ms_host / 1000.0), "unit": "read pairs/s", "h2d_bytes_per_step": R.in_bytes, "d2h_bytes_per_step": int(R.n * 12),
-                    "note": "kj_classify2() with pinned host buffers, chunked H2D/kernel/D2H pipeline inside"}}
+    res = {"value": total * steps / (ms_dev / 1000.0), "ms_per_step": ms_dev / steps, "kernel_ms": kernel_ms, "gpu_launches": int(launches),
+           "e2e": {"value": total * steps / (ms_host / 1000.0), "unit": "read pairs/s", "h2d_bytes_per_step": R.in_bytes, "d2h_bytes_per_step": int(R.n * 12),
+                   "note": "kj_classify2() with pinned host buffers, chunked H2D/kernel/D2H pipeline inside"}}
+    if keep_outputs:
+        res["outputs"] = outputs
+    return res
+
+
+DUMP_SAMPLE = 1 << 20          # reads written by --dump-outputs: 28 MB in all, within the 64 MB bound
+
+
+def dump_outputs(d, outputs):
+    """--dump-outputs: the per-read arrays kj_classify_device2 hands its caller (taxon id, best score / length, dense taxon index; 0xffffffff =
+    unclassified), for the same fixed sample of read indices in every run (seeded, sorted), as float64 / float32 .npy files (every value is exact
+    in that type).  read_index.npy holds the sampled indices into the step's batch."""
+    n = len(outputs["taxon"]); m = min(n, DUMP_SAMPLE)
+    idx = np.arange(n) if m == n else np.sort(np.random.default_rng(20251015).choice(n, m, replace=False))
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "read_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(d, "taxon.npy"), outputs["taxon"][idx].astype(np.float64))
+    np.save(os.path.join(d, "best.npy"), outputs["best"][idx].astype(np.float32))
+    np.save(os.path.join(d, "taxon_index.npy"), outputs["taxon_index"][idx].astype(np.float64))
 
 
 def peak_hbm():
@@ -298,7 +335,7 @@ def peak_hbm():
             return float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
         pass
-    return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+    return 3350.0, "data sheet 3350 GB/s (H100 SXM HBM3; not measured)"
 
 
 def cpu_legs(R, res, mode, db, fmi, nodes, args, n_or=20000):
@@ -350,7 +387,7 @@ def main():
     import torch
     import kaiju_b200 as kb
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device -- the H100 path has no CPU fallback")
     torch.cuda.set_device(local)
     dist = None
     if world > 1:
@@ -366,8 +403,12 @@ def main():
     R = Runner(torch, dist, world, local, *db.reads(7, rank * n, n, 150, True))      # this rank's shard of the job: items [rank*n, (rank+1)*n)
 
     sampler = ClockSampler(local); sampler.start()
-    res = measure(R, clf, args.steps, args.warmup, world)
+    res = measure(R, clf, args.steps, args.warmup, world, keep_outputs=bool(args.dump_outputs))
     sampler.stop_flag = True; sampler.join(timeout=2)
+    outputs = res.pop("outputs", None)
+    if outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, outputs)
+    del outputs
     # untimed: the kaiju2table-style summary -- per-taxon read counts in HBM, one all-reduce across the ranks (SURVEY.md 8e); and the
     # dense indices the ranks gathered map back to the 64-bit ids
     clf.counts_reset(); clf.counts_add_device(R.d_tax.data_ptr(), n); torch.cuda.synchronize()
@@ -387,8 +428,8 @@ def main():
     if dist:   # strong scaling: the 10 M-pair job of ONE GPU split over the ranks (reads [0, n) of the same stream)
         lo, hi = rank * n // world, (rank + 1) * n // world
         RS = Runner(torch, dist, world, local, *db.reads(7, lo, hi - lo, 150, True))
-        ms_s, _ = RS.timed(clf, RS.step_device, max(2, args.steps // 2), 2)
-        strong = {"value": n * max(2, args.steps // 2) / (ms_s / 1000.0), "unit": "read pairs/s", "total_pairs": n, "note": "fixed job of %d pairs split over %d GPUs, device-resident, gather included" % (n, world)}
+        ms_s, _ = RS.timed(clf, RS.step_device, args.steps, 2)
+        strong = {"value": n * args.steps / (ms_s / 1000.0), "unit": "read pairs/s", "total_pairs": n, "note": "fixed job of %d pairs split over %d GPUs, device-resident, gather included" % (n, world)}
         del RS
 
     line = None
@@ -398,7 +439,8 @@ def main():
                 "vs_baseline": None, "dtype": "int64", "data": "synthetic",
                 "config": {"workload": "configs[1]: %s -m 11 (SEG on), %d synthetic PE150 pairs per GPU per step vs synth-viruses .fmi (%d proteins, bwtlen %d)" % (args.mode.upper(), n, args.nprot, clf.bwtlen),
                            "parallelism": "read-sharded x%d, index replicated, NCCL all-gather of uint32 dense taxon indices per step on a side stream" % world if world > 1 else "single GPU",
-                           "l2": "inputs (%.1f GB/step) and index (%.2f GB) exceed the 126 MB L2" % (R.in_bytes / 1e9, clf.index_bytes / 1e9),
+                           "l2": "inputs (%.1f GB/step) and index (%.2f GB) exceed the %d MB L2" % (R.in_bytes / 1e9, clf.index_bytes / 1e9,
+                                                                                                     torch.cuda.get_device_properties(local).L2_cache_size >> 20),
                            "launch": dict(zip(("grid", "block", "dyn_smem"), clf.launch_geometry)),
                            "index_build_ms": clf.index_build_ms,
                            "per_taxon_counts": "%d taxa with reads, counts sum to %d reads (untimed; all-reduce over %d rank(s))" % (len(ids_c) - 1, int(cnt_c.sum()), world)},
@@ -417,7 +459,7 @@ def main():
         mem_tax = R.h_tax.numpy().view(np.uint64).copy() if args.mode == "mem" else None
         try:
             clf.set_params(kb.make_params(other, m=11))
-            sub = measure(R, clf, max(2, args.steps // 2), 3, 1)
+            sub = measure(R, clf, args.steps, 3, 1)
             sub.update({"workload": "configs[2]: %s -e 3 -s 65 -m 11 (E-value 0.01, SEG on), the same %d PE150 pairs vs synth-viruses .fmi" % (other.upper(), n) if other == "greedy" else "MEM -m 11"})
             if not args.skip_cpu:
                 cpu_legs(R, sub, other, db, fmi, nodes, args)
@@ -440,7 +482,7 @@ def main():
 
 
 def large_index(kb, torch, R, clf_base, fmi, nodes, mem_tax, args, local, alg_base):
-    """configs[3]: MEM against a refseq_ref-scale index resident in HBM (see the module docstring)."""
+    """configs[3]: MEM against a large index resident in HBM (see the module docstring)."""
     clf_base.set_params(kb.make_params("mem", m=11))       # (a context that leaves Greedy mode returns its record buffers: HBM for the large index)
     free, total = torch.cuda.mem_get_info()
     copies = max(2, int(round(args.large_rows / clf_base.bwtlen)))
@@ -451,11 +493,11 @@ def large_index(kb, torch, R, clf_base, fmi, nodes, mem_tax, args, local, alg_ba
     big = kb.Classifier(fmi, nodes, device=local, params=kb.make_params("mem", m=11), copies=copies)
     t_create = time.time() - t0
     try:
-        sub = measure(R, big, 2, 3, 1)
+        sub = measure(R, big, args.steps, 3, 1)
         tax = R.h_tax.numpy().view(np.uint64)
         diffs = int((tax != mem_tax).sum()) if mem_tax is not None else None
         peak, peak_src = peak_hbm()
-        sub.update({"workload": "configs[3]: MEM -m 11, the same %d PE150 pairs vs a refseq_ref-scale index: synth-viruses x %d copies = %d BWT rows, %.1f GB resident in HBM (64-bit interval kernels, 192-row rank records)"
+        sub.update({"workload": "configs[3]: MEM -m 11, the same %d PE150 pairs vs a large index: synth-viruses x %d copies = %d BWT rows, %.1f GB resident in HBM (64-bit interval kernels, 192-row rank records)"
                                 % (R.n, copies, big.bwtlen, big.index_bytes / 1e9),
                     "index": {"bwt_rows": big.bwtlen, "sequences": big.nseq, "hbm_bytes": big.index_bytes, "device_build_ms": big.index_build_ms, "create_s": t_create,
                               "built_by": "kj_create_scaled on the device from the 2e8-row .fmi (no host transcode, no suffix sort)"},

@@ -1,4 +1,4 @@
-/* kaiju_b200.h -- C ABI of the B200-native Kaiju classification path (libkaijub200.so).
+/* kaiju_b200.h -- C ABI of the H100-native Kaiju classification path (libkaijub200.so).
  *
  * Drop-in boundary: the reference has no FFI; its seam is the C++ class ConsumerThread
  * (src/ConsumerThread.hpp:64-121): N threads each pop ReadItem* from a queue, classify it against the
@@ -104,7 +104,7 @@ int kj_create(kj_ctx **out, int device, const kj_params *params, const kj_index_
  * kj_create_scaled: the index of the collection in which every sequence of `index` occurs `copies` times in a row -- identical to what
  * kaiju-mkbwt/-mkfmi produce for the K-fold FASTA (identical suffixes are ordered by sequence number), derived on the device without a
  * suffix sort.  With all copies carrying the taxon of their original, MEM results equal those on the base index; it exists to bring
- * refseq_ref-scale indexes (2.7e10 rows, ~126 GB in HBM) onto a GPU for capacity and throughput measurements.  copies = 1 == kj_create. */
+ * indexes of 1e10 rows and more (~47 GB in HBM per 1e10 rows) onto a GPU for capacity and throughput measurements.  copies = 1 == kj_create. */
 int kj_create_scaled(kj_ctx **out, int device, const kj_params *params, const kj_index_view *index, const kj_taxonomy_view *taxonomy, uint32_t copies);
 double kj_index_build_ms(const kj_ctx *ctx);      /* wall time of the index construction inside kj_create / kj_create_scaled */
 /* Device-native index file (SURVEY.md 8f-4): kj_native_index_write() transcodes once (the .fmi + nodes.dmp views as for kj_create) and

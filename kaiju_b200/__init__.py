@@ -1,6 +1,6 @@
-"""kaiju_b200 -- B200-native Kaiju classification path (host-side Python mirror of include/kaiju_b200.h).
+"""kaiju_b200 -- H100-native Kaiju classification path (host-side Python mirror of include/kaiju_b200.h).
 
-The product is the C-ABI shared library ``kaiju_b200/libkaijub200.so`` (CUDA, sm_100a).  This module only
+The product is the C-ABI shared library ``kaiju_b200/libkaijub200.so`` (CUDA, sm_90a).  This module only
 binds it with ctypes; there is no Python or CPU implementation of the path, and importing the binding on a
 machine without the built library raises immediately.
 

@@ -159,7 +159,7 @@ int run_verbose(kj_ctx* ctx, kj_fmi* fmi, const kj_params& P, const std::string&
 
 static void die(const std::string& m) { fprintf(stderr, "Error: %s\n\n", m.c_str()); exit(EXIT_FAILURE); }
 static void usage(const char* prog) {
-    fprintf(stderr, "kaiju-b200 (B200-native classification path of Kaiju)\n\nUsage:\n   %s -t nodes.dmp -f kaiju_db.fmi -i reads.fastq [-j reads2.fastq]\n\n"
+    fprintf(stderr, "kaiju-b200 (H100-native classification path of Kaiju)\n\nUsage:\n   %s -t nodes.dmp -f kaiju_db.fmi -i reads.fastq [-j reads2.fastq]\n\n"
                     "Mandatory arguments:\n   -t FILENAME   Name of nodes.dmp file\n   -f FILENAME   Name of database (.fmi) file\n   -i FILENAME   Name of input file containing reads in FASTA or FASTQ format\n\n"
                     "Optional arguments:\n   -j FILENAME   Name of second input file for paired-end reads\n   -o FILENAME   Name of output file. If not specified, output will be printed to STDOUT\n"
                     "   -z INT        accepted for compatibility (ignored: the GPU replaces the worker threads)\n   -a STRING     Run mode, either \"mem\"  or \"greedy\" (default: greedy)\n"

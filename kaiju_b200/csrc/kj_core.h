@@ -100,9 +100,9 @@ static KJ_DEV void kj_flag_error(KjWarpCtx& cx, uint32_t bit) {
 #endif
 }
 
-// A/B-tested on the B200 (profiles/README.md): one warp's time is dominated by chains of dependent short-latency instructions,
-// so shorter dependence chains beat fewer instructions.  Tried and rejected: two lanes per chain in phase B (-7 %),
-// compaction of low-diversity SEG windows (-10 %), screening several queued fragments at once with two chains per lane (-29 %).
+// Chosen by A/B runs: one warp's time is dominated by chains of dependent short-latency instructions,
+// so shorter dependence chains beat fewer instructions.  Tried and rejected as slower: two lanes per chain in phase B,
+// compaction of low-diversity SEG windows, screening several queued fragments at once with two chains per lane.
 // ---------------------------------------------------------------------------------------------
 // FM index primitives.  IdxT = uint32_t for indexes with bwtlen < 2^32 (all interval arithmetic in 32 bit), uint64_t otherwise.
 // ---------------------------------------------------------------------------------------------
@@ -442,7 +442,7 @@ static KJ_DEV void kj_split_frames(KjWarpCtx& cx, KjQueue& q, const int na1, con
 }
 
 // The same splitting with the four arrays one after the other (one copy of the run logic instead of four interleaved ones: a quarter of the code).
-// Greedy only: there the instruction cache, not the dependent latency of this step, is the scarce resource (profiles/README.md, round 2).  The
+// Greedy only: there the instruction cache, not the dependent latency of this step, is the scarce resource (see kj_warp.h).  The
 // queue slots are filled in another order; the keys (value, reference insertion order) are the same, and only they decide the pop order.
 static KJ_DEV void kj_split_frames_rolled(KjWarpCtx& cx, KjQueue& q, const int na1, const int na2, const int n1, const int n2, const bool greedy, const int nframes) {
     const Warp& w = cx.w; const KjTables& tb = *cx.tb;
@@ -516,7 +516,7 @@ static KJ_DEV void kj_translate_pair(KjWarpCtx& cx, KjQueue& q, const uint8_t* s
         }
     }
     w.sync();
-#ifndef KJ_SPLIT_UNROLLED_GREEDY      // A/B round 2: Greedy +12 % (16.04 vs 14.30 M pairs/s) with the quarter-size splitting code
+#ifndef KJ_SPLIT_UNROLLED_GREEDY      // Greedy is faster with the quarter-size splitting code (A/B)
     if (small_code) kj_split_frames_rolled(cx, q, na1, na2, n1, n2, greedy, 3); else
 #endif
     kj_split_frames(cx, q, na1, na2, n1, n2, greedy, 3);
@@ -556,7 +556,7 @@ static KJ_DEV bool kj_seg_flags(KjWarpCtx& cx, int n, const bool compact) {
             const uint32_t a0 = aw[0], a1 = aw[1], a2 = aw[2], a3 = aw[3];
             const uint32_t w0 = kj_funnel_r(a0, a1, sh), w1 = kj_funnel_r(a1, a2, sh), w2 = kj_funnel_r(a2, a3, sh);
             uint32_t seen = 0;
-#ifndef KJ_NO_GREEDY_COMPACT    // A/B round 2 (with the unified update in kj_seg_trim): Greedy 16.02 -> 16.73 M pairs/s, MEM +0.6 %
+#ifndef KJ_NO_GREEDY_COMPACT    // faster for Greedy in an A/B run (with the unified update in kj_seg_trim), neutral for MEM
             if (compact) { KJ_ROLLED for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); } } else
 #endif
             for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); }
@@ -944,7 +944,7 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
                 if (w.lane == 0) { if (start_la) kj_emu_stats.lookaheads++; else kj_emu_stats.blocks++; }
 #endif
             }
-#ifndef KJ_PROBE     // chains below the scan range as extra bounds: measured -9 % (their rank traffic costs more than the skipped chains save)
+#ifndef KJ_PROBE     // chains below the scan range as extra bounds: slower in an A/B run (their rank traffic costs more than the skipped chains save)
             const int j = jhi - w.lane; const bool act = j >= (int)L - 1; const bool probe = act;
 #else
             const int j = jhi - w.lane; const bool probe = j >= 0; const bool act = j >= (int)L - 1;
@@ -1097,7 +1097,7 @@ static KJ_DEV void kj_protein_fragments(KjWarpCtx& cx, KjQueue& q, const uint8_t
 
 // ---------------------------------------------------------------------------------------------
 // Greedy in two kernels (ROLE 1 = front end, ROLE 2 = search; ROLE 0 = everything in one kernel, as MEM runs).  Greedy is bound by instruction
-// fetch (profiles/README.md, round 2): translation, frame splitting and queue ranking are 6 KB of its hot code that the search does not need.
+// fetch (see kj_warp.h): translation, frame splitting and queue ranking are 6 KB of its hot code that the search does not need.
 // The front end leaves, per item, the four translated arrays and the ranked fragment queue in a record in global memory (1.5 KB for PE150);
 // the search kernel copies the record into the same places of its work space and continues exactly where the single kernel would.
 //   record: [0] uint32 queue length (0xffffffff = unclassified by the length gates), [16] keys, pays, ranks, [..] the aa arrays
@@ -1157,12 +1157,12 @@ static KJ_DEV uint32_t kj_classify_item(KjWarpCtx& cx, const uint8_t* s1, int n1
             if ((!paired && n1 < m3) || (paired && n1 < m3 && n2 < m3)) ok = false;
             else kj_translate_pair(cx, q, s1, n1, n1 >= m3, s2, n2, paired && n2 >= m3, greedy, small_code);   // a short mate is skipped individually (699, 705)
         }
-        if (ok && MODE == 1) kj_queue_sort(cx, q);     // greedy pops every fragment (and many variants): ranking once pays (A/B +9 %); MEM stops after a few pops (A/B -16 %)
+        if (ok && MODE == 1) kj_queue_sort(cx, q);     // greedy pops every fragment (and many variants): ranking once pays (A/B); MEM stops after a few pops (slower with it)
         if (ROLE == 1) {
             // The search would run the SEG gate on every fragment it pops; for most of them the window classes already say "nothing to mask" (kj_seg
             // returns 0 and the fragment is searched as it is).  Decide that here, for every queued fragment, and mark it as checked: the class scan
-            // leaves the search kernel's hot loop (6 % of its instructions, 1.5 KB of its hot code) for this kernel, which has issue slots to spare.
-#ifdef KJ_FRONT_SEG      // A/B round 2 (r2k, front end not yet running beside the search): 17.85 vs 18.50 M pairs/s -- the scan of ALL queued fragments costs more than the popped ones save
+            // leaves the search kernel's hot loop (a few per cent of its instructions and of its hot code) for this kernel, which has issue slots to spare.
+#ifdef KJ_FRONT_SEG      // slower in an A/B run (front end not yet running beside the search): the scan of ALL queued fragments costs more than the popped ones save
             if (ok && MODE == 1 && rp.seg) {
                 KJ_ROLLED
                 for (uint32_t i = 0; i < q.n; i++) {

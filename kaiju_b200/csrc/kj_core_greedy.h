@@ -24,7 +24,7 @@ static KJ_HD uint32_t kj_greedy_scratch_bytes(const KjRunParams& rp) { return rp
 
 struct KjMatch { uint64_t lo; uint32_t len; uint16_t qi, ql; };    // one SI: interval + query position/length
 
-// key(s) = kj_qkey(score, order), 0 = free.  (Keeping the first keys in shared memory was slower: A/B 7.7 vs 8.3 M pairs/s.)
+// key(s) = kj_qkey(score, order), 0 = free.  (Keeping the first keys in shared memory was slower in an A/B run.)
 struct KjVQueue { uint64_t* gkey; KjVariant* v; uint32_t n, live;      // n: high-water mark, live: entries not yet popped (uniform)
     KJ_DEV uint64_t& key(uint32_t s) const { return gkey[s]; } };
 

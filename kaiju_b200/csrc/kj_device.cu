@@ -24,13 +24,13 @@
 
 #define KJ_WARPS_PER_CTA 8
 #ifndef KJ_MIN_BLOCKS
-#define KJ_MIN_BLOCKS 4          // resident CTAs per SM the register allocation is tuned for (ncu: latency-bound, see profiles/)
+#define KJ_MIN_BLOCKS 4          // resident CTAs per SM the register allocation is tuned for (the search is latency-bound; on an H100 (400 W) 4 beat 3 CTAs, 50.6 vs 46.5 M pairs/s MEM)
 #endif
 #ifndef KJ_MIN_BLOCKS_GREEDY_SPLIT
-#define KJ_MIN_BLOCKS_GREEDY_SPLIT 5   // front-end / search kernels of the two-kernel Greedy path: A/B round 2 (r2i) 18.14 vs 17.90 M pairs/s, e2e 17.07 vs 16.41
+#define KJ_MIN_BLOCKS_GREEDY_SPLIT 4   // front-end / search kernels of the two-kernel Greedy path: on an H100 (400 W) 4 CTAs (64 registers) beat 5 (48), 13.8 vs 12.9 M pairs/s
 #endif
 #ifndef KJ_MIN_BLOCKS_GREEDY
-#define KJ_MIN_BLOCKS_GREEDY 4   // A/B round 2 (5 CTAs = 48 registers): 12.0 vs 12.3 M pairs/s -- more warps, but more spill traffic and more instruction-fetch stalls
+#define KJ_MIN_BLOCKS_GREEDY 4   // 5 CTAs (48 registers) was slower in an A/B run: more warps, but more spill traffic and more instruction-fetch stalls
 #endif
 #define KJ_KEPT_SMEM_FIXED 20      // = KJ_KEPT_SMEM of kj_host.cpp (checked at launch: the fixed profile is only used when the layouts agree)
 #define KJ_CHUNK_READS (1u << 20)
@@ -40,7 +40,7 @@
 
 struct KjCtaShared { KjDevIndex ix; KjTables tb; };
 
-// ---- bulk copy (the Blackwell/Hopper copy engine, "TMA" in its 1-D form) of a warp's claimed reads into shared memory: one elected lane
+// ---- bulk copy (the Hopper copy engine, "TMA" in its 1-D form) of a warp's claimed reads into shared memory: one elected lane
 // arms the warp's mbarrier with the byte count and issues cp.async.bulk; the 32 lanes wait on the barrier's phase.  The translation
 // passes then read the bases from shared memory instead of waiting on global loads pass by pass.
 static __device__ __forceinline__ uint32_t kj_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -110,7 +110,7 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
 #ifdef KJ_STAGE
     const bool stage = !GWS && rp.stage != 0;
 #else
-    const bool stage = false;          // measured: -10 % (the larger shared-memory carve-out shrinks the L1 that serves the rank loads), see profiles/README.md
+    const bool stage = false;          // slower in an A/B run: the larger shared-memory carve-out shrinks the L1 that serves the rank loads
 #endif
     uint64_t* mbar = (uint64_t*)(cx.smem + cx.L.mbar_off); uint8_t* stg = cx.smem + cx.L.stage_off; uint32_t phase = 0;
     if (stage) { if (cx.w.lane == 0) kj_mbar_init(mbar, 1); cx.w.sync(); }
@@ -252,11 +252,11 @@ template <class T> static int upload(const std::vector<T>& v, void** d, uint64_t
 
 // Shared-memory work space while three CTAs still fit on an SM; beyond that (mates longer than ~280 bases) the same
 // carve-up is addressed in a global buffer instead, which keeps the grid at full occupancy for any read length.
-// Measured (MEM, kernel-only, M pairs/s, shared vs global): PE150 57.8 vs 45.8, PE250 29.4 (3 CTAs/SM) vs 28.2, PE350 14.3 (2 CTAs/SM) vs 18.3.
+// (A/B, MEM kernel-only: shared memory wins for PE150 and PE250 at 3 CTAs/SM, the global buffer wins for PE350 where only 2 CTAs/SM would fit.)
 #define KJ_SMEM_WS_LIMIT (75u * 1024u)
 // the fixed-profile kernels apply when the batch's carve-up is exactly the compiled-in one
 static bool kj_use_fixed(const KjRunParams& rp) {
-    if (rp.ws_global || rp.mode != 1 || getenv("KJ_NO_FIXED")) return false;      // A/B round 2: Greedy +17 % (14.35 vs 12.26 M pairs/s), MEM -2 % (62.4 vs 63.7): Greedy only
+    if (rp.ws_global || rp.mode != 1 || getenv("KJ_NO_FIXED")) return false;      // A/B: faster for Greedy, slightly slower for MEM: Greedy only
     const KjSmemLayout a = kj_smem_layout(rp), b = kj_smem_layout(kj_fixed_profile(rp.mode));
     return memcmp(&a, &b, sizeof a) == 0 && rp.max_len == 152 && rp.kept_cap_smem == KJ_KEPT_SMEM_FIXED;
 }
@@ -417,8 +417,8 @@ static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, 
     c->H.kmer_k = 0;
     if ((rc = upload_descriptor(c))) return rc;
     { const char* ek = getenv("KJ_KMER_K"); if ((rc = kj_device_build_kmer(c, ek ? atoi(ek) : kj_default_kmer_k(c->H.bwtlen), tot))) return rc; }
-    // MEM runs 4 % faster with the intervals of all 20^7 7-mers (10.2 GB below 2^32 rows): one look-up replaces the first LF step of every chain, the one
-    // with all 32 lanes alive.  Greedy loses 2 % with it (its seeds rarely get that far), so it keeps the 6-mer table: two descriptors, one index.
+    // MEM runs faster with the intervals of all 20^7 7-mers (10.2 GB below 2^32 rows): one look-up replaces the first LF step of every chain, the one
+    // with all 32 lanes alive.  Greedy loses with it (its seeds rarely get that far), so it keeps the 6-mer table: two descriptors, one index.
     // Only where HBM is plentiful: narrow indexes, and the two level buffers of the construction (41 GB) must fit next to the index.
     if (!c->H.wide && c->H.kmer_k == 6 && !kj_transient_ctx && !getenv("KJ_KMER_K") && !getenv("KJ_NO_KMER7")) {
         size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));
@@ -522,7 +522,7 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     const uint32_t pstride = split ? kj_prep_stride(rp) : 0u; uint64_t sub = n;
     if (split) {
         // records of one sub-batch per buffer; two buffers per slot (the front end of sub-batch b+1 runs in the tail of the search of sub-batch b).
-        // Up to 8 GB per buffer where HBM is plentiful: fewer, longer search launches (750 k vs 3 M pairs per launch: 17.9 vs 18.3 M pairs/s)
+        // Up to 8 GB per buffer where HBM is plentiful: fewer, longer search launches (3 M rather than 750 k pairs per launch was faster in an A/B run)
         uint64_t per_buf = c->prep_bytes / 4;
         if (per_buf < (8ull << 30) && per_buf < n * (uint64_t)pstride) {       // (re)allocate: what this launch needs, at least 1 GB, at most 8 GB or 1/16 of the free memory
             size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to)); fr += c->prep_bytes;
@@ -546,8 +546,8 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
                         else if (rp.ws_global) KJ_LAUNCH3(M, T, true, false, false, 0, 0, n); else if (fixed) KJ_LAUNCH3(M, T, false, true, false, 0, 0, n); else KJ_LAUNCH3(M, T, false, false, false, 0, 0, n)
 #define KJ_LAUNCH_SPLIT(T, R, B0, B1) if (fixed) KJ_LAUNCH3(1, T, false, true, false, R, B0, B1); else KJ_LAUNCH3(1, T, false, false, false, R, B0, B1)
     uint8_t* pbuf = nullptr; unsigned long long* ctr = c->d_counter + slot; cudaStream_t kst = st; int kgrid = grid;
-    // (A/B r2l: a search grid that leaves one CTA slot per SM to the front end of the next sub-batch loses 9 % -- 32 instead of 40 search warps per SM cost
-    // more than the hidden front end (8 % of the kernel time) gives back; KJ_SPLIT_LEAVE_SLOT keeps the experiment)
+    // (A/B: a search grid that leaves one CTA slot per SM to the front end of the next sub-batch is slower -- 32 instead of 40 search warps per SM cost
+    // more than the hidden front end gives back; KJ_SPLIT_LEAVE_SLOT keeps the experiment)
     const int per_sm = grid / c->sm_count; const int sgrid = (per_sm >= 3 && getenv("KJ_SPLIT_LEAVE_SLOT")) ? c->sm_count * (per_sm - 1) : grid;
     if (split) {
         // front end on the slot's own stream, search on the caller's: F(b) -> S(b) through ev_f, S(b) -> F(b+2) (same buffer) through ev_s

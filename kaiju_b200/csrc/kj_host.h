@@ -41,7 +41,7 @@ int kj_build_host_meta(const kj_index_view& v, const kj_taxonomy_view& t, uint32
 // SA intervals of all 20^k k-mers over the 20 residue letters (exactness-preserving shortcut for the first k LF steps)
 void kj_build_kmer_table(KjHostIndex& H, int k);
 // k of the k-mer interval table: 6 letters (20^6 entries, 0.5-1 GB) once the index is large enough that 6-mers are mostly present
-// (A/B on the 2e8-row index: 63.5 vs 61.9 M pairs/s MEM), 5 letters (26-51 MB) below that
+// (faster for MEM on the 2e8-row index in an A/B run), 5 letters (26-51 MB) below that
 static inline int kj_default_kmer_k(uint64_t bwtlen) { return bwtlen >= 50000000ull ? 6 : 5; }
 // device-native index file (SURVEY.md 8f-4): the transcoded arrays as they are uploaded, so that loading is one sequential read
 int kj_host_index_write(const KjHostIndex& H, const char* path);

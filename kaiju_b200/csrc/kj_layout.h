@@ -21,9 +21,9 @@
 
 // Two record layouts, chosen per index at load time:
 //   narrow (bwtlen < 2^32, 32-bit interval kernels): 16-byte records per 64 rows  { hdr = C[c] + #c before the block, w0 = one-hot bitmap }
-//          -> one 16-byte load + one popcount per rank query, no division; 5.25 B per BWT row (measured +6 % over the 192-row layout)
+//          -> one 16-byte load + one popcount per rank query, no division; 5.25 B per BWT row (faster than the 192-row layout where both fit)
 //   wide   (bwtlen >= 2^32, 64-bit interval kernels): 32-byte records per 192 rows { hdr (40-bit count | popc(w0) | popc(w0)+popc(w1)), w0, w1, w2 }
-//          -> 3.5 B per row: a refseq_ref-scale index (2.7e10 rows) takes 95 GB of the 180 GB HBM instead of 142 GB
+//          -> 3.5 B per row: an index of 1.2e10 rows takes 42 GB of the 80 GB HBM instead of 63 GB
 #define KJ_RANK_ROWS_NARROW 64
 #define KJ_RANK_ROWS_WIDE 192
 #define KJ_RANK_WORDS_NARROW 2

@@ -1,6 +1,6 @@
 // kj_warp.h -- the warp-collective vocabulary the classification kernels are written in.
 //
-// Device build (nvcc, sm_100a): thin wrappers over the SIMT intrinsics (full-mask collectives).
+// Device build (nvcc, sm_90a): thin wrappers over the SIMT intrinsics (full-mask collectives).
 // KJ_EMU build (g++, tests/emu only): the same member functions implemented on a 32-fiber
 // cooperative scheduler, so the *identical* kernel source (kj_core.h) can be exercised on a machine
 // without a GPU.  The emulator is test infrastructure; the product library never compiles with KJ_EMU.
@@ -50,7 +50,7 @@ struct Warp {
 #define KJ_DEV __device__ __forceinline__
 #define KJ_HD __host__ __device__ __forceinline__
 #define KJ_FULL 0xffffffffu
-// Code size is a first-order cost here (the Greedy kernel stalled 58 % of its time on instruction fetch, profiles/README.md):
+// Code size is a first-order cost here (the Greedy kernel stalls on instruction fetch when its hot loop outgrows the instruction cache):
 // loops are kept rolled unless unrolling was measured to pay, and cold paths are real functions.
 #define KJ_ROLLED _Pragma("unroll 1")
 #define KJ_NOINLINE static __device__ __noinline__

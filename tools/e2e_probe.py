@@ -1,5 +1,6 @@
 import os, sys, time, numpy as np, torch
-sys.path.insert(0, "/root/repo"); sys.path.insert(0, "/root/repo/tests")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import kaiju_b200 as kb
 from helpers import SynthDB, build_fmi
 wd = "/tmp/kjbench"; os.makedirs(wd, exist_ok=True)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Developer tool: static SASS size of the kernels in a cubin, attributed to source functions through the -lineinfo table
-(the instruction-cache footprint is what limits the Greedy kernel: profiles/README.md).  Usage: tools/sass_size.py <cubin> [kernel-substring]"""
+(the instruction-cache footprint is what limits the Greedy kernel: DESIGN.md §3).  Usage: tools/sass_size.py <cubin> [kernel-substring]"""
 import re, subprocess, sys, os
 cubin = sys.argv[1]; want = sys.argv[2] if len(sys.argv) > 2 else "kj_classify_kernelILi1EjLb0"
 out = subprocess.run(["nvdisasm", "--print-line-info-inline", cubin], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL).stdout.decode(errors="replace")

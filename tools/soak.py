@@ -1,7 +1,7 @@
 """Developer tool (CPU only): the UNMODIFIED reference binary (oracle/_ref/kaiju) against the kernel logic on the CPU warp emulator, directly,
 on a fresh seeded workload of N read items per configuration (PE150, SE100, PE250 x MEM / Greedy parameter sets).  Usage: python tools/soak.py 1000000"""
 import sys, time, numpy as np, ctypes as C, os, tempfile
-sys.path.insert(0, '/root/repo/tests')
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 from conftest import ROOT
 from helpers import *
 from test_kernel_logic_emulated import KjParams
