@@ -226,11 +226,12 @@ struct kj_ctx {
     uint64_t index_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;
     // run state
     unsigned long long* d_counter = nullptr; uint32_t* d_err = nullptr; unsigned int* d_maxlen = nullptr;
-    KjKept* d_spill = nullptr; size_t spill_bytes = 0; uint8_t* d_gscratch = nullptr; size_t gscratch_bytes_total = 0;
+    // per-warp global scratch, one allocation per pipeline slot (ensure_scratch): spill entries, Greedy variant ring, work space of long reads
+    KjKept* d_spill[2] = {nullptr, nullptr}; size_t spill_bytes[2] = {0, 0}; uint8_t* d_gscratch[2] = {nullptr, nullptr}; size_t gscratch_bytes_total[2] = {0, 0};
     double* d_evbreaks = nullptr; uint32_t n_evbreaks = 0; uint64_t* d_quirk = nullptr;
     unsigned long long* d_counts = nullptr; unsigned long long* d_counts_pending = nullptr; uint32_t n_counts = 0, n_present = 0;   // per-taxon read counts (+1 slot: unclassified)
     uint32_t variant_boost = 1;    // Greedy variant-ring capacity multiplier, raised after an overflow (flag 4) so that a retry succeeds
-    uint8_t* d_ws = nullptr; size_t ws_bytes = 0;
+    uint8_t* d_ws[2] = {nullptr, nullptr}; size_t ws_bytes[2] = {0, 0};
     uint8_t* d_prep = nullptr; size_t prep_bytes = 0;      // prepared-item records of the two-kernel Greedy path (two slots x two buffers)
     cudaStream_t fstream[2] = {nullptr, nullptr}; cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_f[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}}, ev_s[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // front-end stream + hand-over events per slot
     cudaStream_t stream[2] = {nullptr, nullptr}; cudaEvent_t ev_a = nullptr, ev_b = nullptr;
@@ -305,14 +306,22 @@ static int configure_launch(kj_ctx* c, KjRunParams& rp, size_t& smem, int& grid,
     return KJ_OK;
 }
 
-static int ensure_scratch(kj_ctx* c, const KjRunParams& rp, int grid) {
-    size_t warps = (size_t)grid * KJ_WARPS_PER_CTA * 2;   // two pipeline slots may be in flight
-    size_t need = warps * rp.scratch_entries * sizeof(KjKept);
-    if (need > c->spill_bytes) { if (c->d_spill) cudaFree(c->d_spill); c->d_spill = nullptr; CK(cudaMalloc((void**)&c->d_spill, need)); c->spill_bytes = need; }
-    size_t gneed = warps * (size_t)kj_greedy_scratch_bytes(rp);
-    if (gneed > c->gscratch_bytes_total) { if (c->d_gscratch) cudaFree(c->d_gscratch); c->d_gscratch = nullptr; CK(cudaMalloc((void**)&c->d_gscratch, gneed)); c->gscratch_bytes_total = gneed; }
-    size_t wneed = rp.ws_global ? warps * (size_t)kj_smem_layout(rp).total : 0;
-    if (wneed > c->ws_bytes) { if (c->d_ws) cudaFree(c->d_ws); c->d_ws = nullptr; CK(cudaMalloc((void**)&c->d_ws, wneed)); c->ws_bytes = wneed; }
+// Two pipeline slots may be in flight, and their launches may have different run parameters (kj_classify_files derives them from each
+// batch's longest read): each slot has its own allocations, sized and grown from that slot's launch alone.  Carving both slots out of one
+// buffer at offsets computed from the current launch's parameters would let a launch with a smaller per-warp size land inside the region
+// the other slot's kernel is still using.  A slot's buffers are only replaced when its own previous work is complete; the cudaFree of the
+// old buffer also waits for the other slot's kernels.
+// Within one slot, the front-end kernel of the two-kernel Greedy path (ROLE 1) runs beside the search kernel (ROLE 2) of the previous
+// sub-batch; it touches neither the spill entries nor the variant ring (translation, queue ranking and the record store only use the
+// shared-memory work space), and the split path never uses the global work space, so the two share the slot's scratch safely.
+static int ensure_scratch(kj_ctx* c, int slot, const KjRunParams& rp, int grid) {
+    const size_t warps = (size_t)grid * KJ_WARPS_PER_CTA;
+    const size_t need = warps * rp.scratch_entries * sizeof(KjKept);
+    if (need > c->spill_bytes[slot]) { if (c->d_spill[slot]) cudaFree(c->d_spill[slot]); c->d_spill[slot] = nullptr; c->spill_bytes[slot] = 0; CK(cudaMalloc((void**)&c->d_spill[slot], need)); c->spill_bytes[slot] = need; }
+    const size_t gneed = warps * (size_t)kj_greedy_scratch_bytes(rp);
+    if (gneed > c->gscratch_bytes_total[slot]) { if (c->d_gscratch[slot]) cudaFree(c->d_gscratch[slot]); c->d_gscratch[slot] = nullptr; c->gscratch_bytes_total[slot] = 0; CK(cudaMalloc((void**)&c->d_gscratch[slot], gneed)); c->gscratch_bytes_total[slot] = gneed; }
+    const size_t wneed = rp.ws_global ? warps * (size_t)kj_smem_layout(rp).total : 0;
+    if (wneed > c->ws_bytes[slot]) { if (c->d_ws[slot]) cudaFree(c->d_ws[slot]); c->d_ws[slot] = nullptr; c->ws_bytes[slot] = 0; CK(cudaMalloc((void**)&c->d_ws[slot], wneed)); c->ws_bytes[slot] = wneed; }
     return KJ_OK;
 }
 
@@ -485,7 +494,7 @@ extern "C" void kj_destroy(kj_ctx* c) {
     kj_files_state_free(c->files); c->files = nullptr;
     if (c->d_ix_mem) cudaFree(c->d_ix_mem); if (c->d_kmer_mem) cudaFree(c->d_kmer_mem); if (c->d_prep) cudaFree(c->d_prep);
     void* ptrs[] = {c->d_rank, c->d_letters, c->d_sa_tax, c->d_seq_tax, c->d_tax_parent, c->d_tax_depth, c->d_tax_id, c->d_lnfact, c->d_kmer, c->d_tables, c->d_ix,
-                    c->d_counter, c->d_err, c->d_maxlen, c->d_spill, c->d_gscratch, c->d_evbreaks, c->d_ws, c->d_counts, c->d_counts_pending, c->d_quirk, c->d_tax[0], c->d_tax[1], c->d_best[0], c->d_best[1],
+                    c->d_counter, c->d_err, c->d_maxlen, c->d_spill[0], c->d_spill[1], c->d_gscratch[0], c->d_gscratch[1], c->d_evbreaks, c->d_ws[0], c->d_ws[1], c->d_counts, c->d_counts_pending, c->d_quirk, c->d_tax[0], c->d_tax[1], c->d_best[0], c->d_best[1],
                     c->d_seq[0][0], c->d_seq[0][1], c->d_seq[1][0], c->d_seq[1][1], c->d_off[0][0], c->d_off[0][1], c->d_off[1][0], c->d_off[1][1],
                     c->d_ids[0], c->d_ids[1], c->d_nids[0], c->d_nids[1], c->d_sa_acc, c->d_seq_acc, c->d_acc[0], c->d_acc[1], c->d_nacc[0], c->d_nacc[1],
                     c->d_frag[0], c->d_frag[1], c->d_fraglen[0], c->d_fraglen[1]};
@@ -510,10 +519,9 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     rp.variant_cap *= c->variant_boost;
     const bool verbose = d_ids || d_acc || d_frag;
     size_t smem; int grid; int rc = configure_launch(c, rp, smem, grid, verbose); if (rc) return rc;
-    rc = ensure_scratch(c, rp, grid); if (rc) return rc;
+    rc = ensure_scratch(c, slot, rp, grid); if (rc) return rc;
     c->grid = grid; c->smem_bytes = smem;
     if (time_it) CK(cudaEventRecord(c->ev_a, st));
-    const size_t warps = (size_t)grid * KJ_WARPS_PER_CTA;
     const KjSmemLayout lay = kj_smem_layout(rp);
     const bool fixed = !verbose && kj_use_fixed(rp);
     const KjDevIndex* dix = (rp.mode == 0 && c->d_ix_mem && rp.m >= (uint32_t)c->kmer_k_mem) ? c->d_ix_mem : c->d_ix;
@@ -538,9 +546,7 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
         sub = std::min(sub, n);
     }
 #define KJ_ARGS(B0, B1) dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, (uint64_t)(B1), d_tax, d_best, d_ids, d_nids, d_compact, \
-            ctr, c->d_spill + (size_t)slot * warps * rp.scratch_entries, \
-            c->d_gscratch + (size_t)slot * warps * kj_greedy_scratch_bytes(rp), kj_greedy_scratch_bytes(rp), \
-            rp.ws_global ? c->d_ws + (size_t)slot * warps * kj_smem_layout(rp).total : nullptr, d_count_dst, c->d_err, d_acc, d_nacc, d_frag, frag_stride, d_fraglen, pbuf, pstride, (uint64_t)(B0)
+            ctr, c->d_spill[slot], c->d_gscratch[slot], kj_greedy_scratch_bytes(rp), rp.ws_global ? c->d_ws[slot] : nullptr, d_count_dst, c->d_err, d_acc, d_nacc, d_frag, frag_stride, d_fraglen, pbuf, pstride, (uint64_t)(B0)
 #define KJ_LAUNCH3(M, T, G, F, V, R, B0, B1) kj_classify_kernel<M, T, G, F, V, R><<<kgrid, KJ_WARPS_PER_CTA * 32, smem, kst>>>(KJ_ARGS(B0, B1))
 #define KJ_LAUNCH(M, T) if (verbose) { if (rp.ws_global) KJ_LAUNCH3(M, T, true, false, true, 0, 0, n); else KJ_LAUNCH3(M, T, false, false, true, 0, 0, n); } \
                         else if (rp.ws_global) KJ_LAUNCH3(M, T, true, false, false, 0, 0, n); else if (fixed) KJ_LAUNCH3(M, T, false, true, false, 0, 0, n); else KJ_LAUNCH3(M, T, false, false, false, 0, 0, n)
