@@ -21,14 +21,12 @@
 // per-warp shared-memory carve-up
 // ---------------------------------------------------------------------------------------------
 #define KJ_SEG_CAP(max_frag) ((max_frag) / 4u + 8u)
-#ifndef KJ_CLAIM
-#define KJ_CLAIM 4               // read items claimed per atomic by a warp
-#endif
 struct KjKept { uint64_t lo; uint32_t len; uint32_t aux; };     // one suffix interval (an SI of bwt.h:25-34)
 
+// (member order: the kernels read these from the parameter bank in 8-byte pairs; accs_off and total are read together)
 struct KjSmemLayout {
     uint32_t qkey_off, qpay_off, kept_off, res_off, res2_off, pre_off, ids_off, qord_off, aa_off, aa_stride, frag_off, hflag_off,
-             segcnt_off, seghist_off, segs_off, stage_off, stage_stride, mbar_off, accs_off, total;
+             segcnt_off, seghist_off, accs_off, total, segs_off;
 #if defined(KJ_EMU)
     uint32_t guard[16], nguard;         // emulator only: 64-byte red zones between the sub-arrays, checked after every read item
 #endif
@@ -71,9 +69,6 @@ static KJ_HD KjSmemLayout kj_smem_layout(const KjRunParams& p) {
     }
     o = u + (seg_bytes > g_bytes ? seg_bytes : g_bytes);
     KJ_GUARD(L, o)
-    // staging area of the claimed reads' bases (cp.async.bulk target: 16-byte aligned) + the warp's mbarrier
-    L.stage_off = L.stage_stride = L.mbar_off = 0;
-    if (p.stage) { o = kj_align(o, 16); L.mbar_off = o; o += 16u; L.stage_off = o; L.stage_stride = kj_align(KJ_CLAIM * p.max_len + 32u, 16); o += 2u * L.stage_stride; }
     L.total = kj_align(o, 16);
     return L;
 }
@@ -141,23 +136,10 @@ static KJ_DEV IdxT kj_rank_at(const uint64_t* base, IdxT k) {
 static KJ_DEV const uint64_t* kj_letter_base(const KjDevIndex& ix, uint32_t c) { return ix.rank_base[c]; }
 template <class IdxT>
 static KJ_DEV IdxT kj_rank(const KjDevIndex& ix, uint32_t c, IdxT k) { return kj_rank_at<IdxT>(kj_letter_base(ix, c), k); }
-// The LF step of the 32-bit kernels as a real function (Greedy, -DKJ_GREEDY_OOL: the step is inlined at five sites of its hot loop, ~30 instructions each;
-// the call costs ~20 cycles next to a ~700-cycle memory round trip, the instruction cache is what Greedy is short of).  Returns nhi << 32 | nlo.
-KJ_NOINLINE uint64_t kj_lf_step32_fn(const uint64_t* base, uint32_t lo, uint32_t hi) {
-    const uint32_t nlo = kj_rank_at<uint32_t>(base, lo), nhi = kj_rank_at<uint32_t>(base, hi);
-    return ((uint64_t)nhi << 32) | (uint64_t)nlo;
-}
 // UpdateSI (bwt.c:160-173)
-template <class IdxT, bool OOL = false>
+template <class IdxT>
 static KJ_DEV bool kj_update_si(const KjDevIndex& ix, uint32_t c, IdxT& lo, IdxT& hi) {
     const uint64_t* base = kj_letter_base(ix, c);
-#ifdef KJ_GREEDY_OOL
-    if (OOL && sizeof(IdxT) == 4) {
-        const uint64_t r = kj_lf_step32_fn(base, (uint32_t)lo, (uint32_t)hi); const uint32_t a = (uint32_t)r, b = (uint32_t)(r >> 32);
-        if (a >= b) return false;
-        lo = (IdxT)a; hi = (IdxT)b; return true;
-    }
-#endif
     IdxT nlo = kj_rank_at<IdxT>(base, lo), nhi = kj_rank_at<IdxT>(base, hi);
     // the reference's checkpoint quirk (indexes with bwtlen = m * 2^16 only, kj_host.cpp): the last 129 positions rank lower by a per-letter
     // constant.  Such indexes are routed to the 64-bit kernels, so the 32-bit ones do not carry the test.
@@ -196,9 +178,7 @@ static KJ_DEV uint32_t kj_sa_taxon(const KjDevIndex& ix, uint64_t k) {
 //   phase B: the surviving chains are completed a few at a time in descending j, replaying the reference's
 //            sequential rules (growing L, `if (i<=1) break`) between groups.
 // ---------------------------------------------------------------------------------------------
-#ifndef KJ_PHASE_A_LETTERS
 #define KJ_PHASE_A_LETTERS 9      // letters matched in phase A (k-mer + single steps)
-#endif
 // chain state: OPEN = alive but not finished (phase-A survivor); EXACT = finished, i = leftmost start of the match ending at j and
 // [lo,hi) its interval; KDEAD = failed inside the k-mer look-up: the match is shorter than k letters, its start lies in [j-k+2, j+1]
 #define KJ_ST_OPEN 0
@@ -210,7 +190,7 @@ struct KjEmuStats { unsigned long long rounds, round_steps, lane_steps, chains, 
 extern thread_local KjEmuStats kj_emu_stats;
 #endif
 
-template <class IdxT, bool OOL = false>
+template <class IdxT>
 static KJ_DEV void kj_chain_start(const KjDevIndex& ix, const uint8_t* frag, int j, uint32_t Lmin, KjChain<IdxT>& ch) {
     const int k = ix.kmer_k; int i = j; int budget = KJ_PHASE_A_LETTERS - 1;
     ch.st = KJ_ST_OPEN;
@@ -227,24 +207,24 @@ static KJ_DEV void kj_chain_start(const KjDevIndex& ix, const uint8_t* frag, int
         const uint32_t c = frag[j]; ch.lo = (IdxT)ix.C[c]; ch.hi = (IdxT)ix.C[c + 1];      // InitialSI (bwt.c:146-152)
     }
     KJ_ROLLED
-    while (i > 0 && budget > 0) { if (!kj_update_si<IdxT, OOL>(ix, frag[i - 1], ch.lo, ch.hi)) { ch.st = KJ_ST_EXACT; break; } i--; budget--; }
+    while (i > 0 && budget > 0) { if (!kj_update_si<IdxT>(ix, frag[i - 1], ch.lo, ch.hi)) { ch.st = KJ_ST_EXACT; break; } i--; budget--; }
     if (i == 0) ch.st = KJ_ST_EXACT;
     ch.i = i;
 }
-template <class IdxT, bool OOL = false>
+template <class IdxT>
 static KJ_DEV void kj_chain_finish(const KjDevIndex& ix, const uint8_t* frag, KjChain<IdxT>& ch) {
     int i = ch.i;
     KJ_ROLLED
-    while (i > 0) { if (!kj_update_si<IdxT, OOL>(ix, frag[i - 1], ch.lo, ch.hi)) break; i--; }
+    while (i > 0) { if (!kj_update_si<IdxT>(ix, frag[i - 1], ch.lo, ch.hi)) break; i--; }
     ch.i = i; ch.st = KJ_ST_EXACT;
 }
 // complete the selected chains (one lane each)
-template <class IdxT, bool OOL = false>
+template <class IdxT>
 static KJ_DEV void kj_finish_selected(const Warp& w, const KjDevIndex& ix, const uint8_t* frag, bool sel, KjChain<IdxT>& ch) {
 #if defined(KJ_EMU)
     const int i0 = ch.i;
 #endif
-    if (sel) kj_chain_finish<IdxT, OOL>(ix, frag, ch);
+    if (sel) kj_chain_finish<IdxT>(ix, frag, ch);
     w.sync();
 #if defined(KJ_EMU)
     { const uint32_t st = sel ? (uint32_t)(i0 - ch.i) + 1u : 0u; const uint32_t mx = warp_max_u32(w, st); const uint32_t nsel = (uint32_t)kj_popc(w.ballot(sel));
@@ -266,16 +246,16 @@ static KJ_DEV void kj_finish_selected(const Warp& w, const KjDevIndex& ix, const
 template <class IdxT>
 static KJ_DEV int kj_chain_lbval(const KjChain<IdxT>& ch, int j, int kk) { return ch.st == KJ_ST_EXACT ? ch.i : (j - kk + 2 > 0 ? j - kk + 2 : 0); }
 template <class IdxT>
-static KJ_DEV int kj_chain_lb(const Warp& w, const KjChain<IdxT>& ch, bool probe, int j, int kk, int lb_ext) {
-    const uint32_t inf = w.ballot(probe && ch.st != KJ_ST_OPEN);
+static KJ_DEV int kj_chain_lb(const Warp& w, const KjChain<IdxT>& ch, bool ran, int j, int kk, int lb_ext) {
+    const uint32_t inf = w.ballot(ran && ch.st != KJ_ST_OPEN);
     const uint32_t below = w.lane < 31 ? inf & ~((2u << w.lane) - 1u) : 0u;
     const int v = w.shfl(kj_chain_lbval<IdxT>(ch, j, kk), below ? kj_ffs(below) - 1 : 0);
     return below ? v : lb_ext;
 }
 // the bound a block hands to the block above it: lbval of its first ended chain (0 if it has none)
 template <class IdxT>
-static KJ_DEV int kj_block_lb_ext(const Warp& w, const KjChain<IdxT>& ch, bool probe, int j, int kk) {
-    const uint32_t inf = w.ballot(probe && ch.st != KJ_ST_OPEN);
+static KJ_DEV int kj_block_lb_ext(const Warp& w, const KjChain<IdxT>& ch, bool ran, int j, int kk) {
+    const uint32_t inf = w.ballot(ran && ch.st != KJ_ST_OPEN);
     const int v = w.shfl(kj_chain_lbval<IdxT>(ch, j, kk), inf ? kj_ffs(inf) - 1 : 0);
     return inf ? v : 0;
 }
@@ -290,9 +270,7 @@ static KJ_DEV uint32_t kj_prefix_min_excl(const Warp& w, uint32_t v, uint32_t in
     const uint32_t e = w.shfl(v, w.lane - 1);
     return w.lane == 0 ? init : (e < init ? e : init);
 }
-#ifndef KJ_GROUP_LATE
 #define KJ_GROUP_LATE 8            // chains completed per round once the first round (segment tops only) did not settle a block
-#endif
 
 // ---------------------------------------------------------------------------------------------
 // fragment queue (std::multimap<unsigned,Fragment*,greater>, ConsumerThread.hpp:83): highest key first,
@@ -516,10 +494,8 @@ static KJ_DEV void kj_translate_pair(KjWarpCtx& cx, KjQueue& q, const uint8_t* s
         }
     }
     w.sync();
-#ifndef KJ_SPLIT_UNROLLED_GREEDY      // Greedy is faster with the quarter-size splitting code (A/B)
-    if (small_code) kj_split_frames_rolled(cx, q, na1, na2, n1, n2, greedy, 3); else
-#endif
-    kj_split_frames(cx, q, na1, na2, n1, n2, greedy, 3);
+    if (small_code) kj_split_frames_rolled(cx, q, na1, na2, n1, n2, greedy, 3);      // Greedy is faster with the quarter-size splitting code (A/B)
+    else kj_split_frames(cx, q, na1, na2, n1, n2, greedy, 3);
 }
 
 // copy the characters of item (arr,start,len) into the contiguous fragment buffer
@@ -556,10 +532,9 @@ static KJ_DEV bool kj_seg_flags(KjWarpCtx& cx, int n, const bool compact) {
             const uint32_t a0 = aw[0], a1 = aw[1], a2 = aw[2], a3 = aw[3];
             const uint32_t w0 = kj_funnel_r(a0, a1, sh), w1 = kj_funnel_r(a1, a2, sh), w2 = kj_funnel_r(a2, a3, sh);
             uint32_t seen = 0;
-#ifndef KJ_NO_GREEDY_COMPACT    // faster for Greedy in an A/B run (with the unified update in kj_seg_trim), neutral for MEM
-            if (compact) { KJ_ROLLED for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); } } else
-#endif
-            for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); }
+            // compact (rolled): faster for Greedy in an A/B run (with the unified update in kj_seg_trim), neutral for MEM
+            if (compact) { KJ_ROLLED for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); } }
+            else for (int t = 0; t < 4; t++) { seen |= 1u << ((w0 >> (8 * t)) & 0xffu); seen |= 1u << ((w1 >> (8 * t)) & 0xffu); seen |= 1u << ((w2 >> (8 * t)) & 0xffu); }
             if (kj_popc(seen) < 8) {
                 int32_t x = 0;
                 KJ_ROLLED
@@ -665,9 +640,6 @@ KJ_NOINLINE uint32_t kj_seg_trim(const Warp w, uint8_t* scratch, const uint8_t* 
             #define KJ_SEG_ADD(letter) { uint32_t a_ = (letter) - 1u; uint32_t c_ = cnt[a_ * 32 + w.lane]; \
                 if (c_ > 0) { uint8_t h_ = --hist[c_ * 32 + w.lane]; if (h_ == 0) { if (c_ < 64) m0 &= ~(1ull << c_); else m1 &= ~(1ull << (c_ - 64)); } } else nz++; \
                 cnt[a_ * 32 + w.lane] = (uint8_t)(c_ + 1); hist[(c_ + 1) * 32 + w.lane]++; if (c_ + 1 < 64) m0 |= 1ull << (c_ + 1); else m1 |= 1ull << (c_ + 1 - 64); }
-            #define KJ_SEG_DEL(letter) { uint32_t a_ = (letter) - 1u; uint32_t c_ = cnt[a_ * 32 + w.lane]; \
-                { uint8_t h_ = --hist[c_ * 32 + w.lane]; if (h_ == 0) { if (c_ < 64) m0 &= ~(1ull << c_); else m1 &= ~(1ull << (c_ - 64)); } } \
-                cnt[a_ * 32 + w.lane] = (uint8_t)(c_ - 1); if (c_ > 1) { hist[(c_ - 1) * 32 + w.lane]++; if (c_ - 1 < 64) m0 |= 1ull << (c_ - 1); else m1 |= 1ull << (c_ - 1 - 64); } else nz--; }
             KJ_ROLLED
             for (int t = 0; t < len; t++) KJ_SEG_ADD(s[t]);
             KJ_ROLLED
@@ -688,7 +660,6 @@ KJ_NOINLINE uint32_t kj_seg_trim(const Warp w, uint8_t* scratch, const uint8_t* 
                 if (nz < 20) ans1 = kj_dsub(ans1, lnf[20 - nz]);
                 double prob = kj_dsub(kj_dadd(ans1, ans2), kj_dmul((double)len, 2.9957322735539909));
                 if (prob < my_prob) { my_prob = prob; my_i = i; }
-#ifndef KJ_NO_GREEDY_COMPACT
                 // one update body for "remove s[i]" and "add s[i+len]" (half the code of the two specialised ones)
                 if (i + len < n2) {
                     KJ_ROLLED
@@ -699,12 +670,8 @@ KJ_NOINLINE uint32_t kj_seg_trim(const Warp w, uint8_t* scratch, const uint8_t* 
                         if (n_ > 0) { hist[n_ * 32 + w.lane]++; if (n_ < 64) m0 |= 1ull << n_; else m1 |= 1ull << (n_ - 64); } else nz--;
                     }
                 }
-#else
-                if (i + len < n2) { KJ_SEG_DEL(s[i]); KJ_SEG_ADD(s[i + len]); }
-#endif
             }
             #undef KJ_SEG_ADD
-            #undef KJ_SEG_DEL
         }
         w.sync();
         // arg-min over lanes, lowest lane (longest window) wins ties
@@ -932,11 +899,7 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
         for (;;) {
             if (jstart >= 0) {                                                              // phase A of the block whose top end position is jstart
                 KjChain<IdxT> t; t.lo = 0; t.hi = 0; t.i = 0; t.st = KJ_ST_EXACT;
-#ifndef KJ_PROBE
                 if (jstart - w.lane >= (int)L - 1 || (start_la && jstart - w.lane >= 0)) kj_chain_start<IdxT>(ix, frag, jstart - w.lane, rp.m, t);
-#else
-                if (jstart - w.lane >= 0) kj_chain_start<IdxT>(ix, frag, jstart - w.lane, rp.m, t);
-#endif
                 w.sync();
                 if (start_la) { nxt = t; have_nxt = true; } else { cur = t; round = 0; }
                 jstart = -1;
@@ -944,11 +907,8 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
                 if (w.lane == 0) { if (start_la) kj_emu_stats.lookaheads++; else kj_emu_stats.blocks++; }
 #endif
             }
-#ifndef KJ_PROBE     // chains below the scan range as extra bounds: slower in an A/B run (their rank traffic costs more than the skipped chains save)
-            const int j = jhi - w.lane; const bool act = j >= (int)L - 1; const bool probe = act;
-#else
-            const int j = jhi - w.lane; const bool probe = j >= 0; const bool act = j >= (int)L - 1;
-#endif
+            // (chains below the scan range as extra bounds were slower in an A/B run: their rank traffic costs more than the skipped chains save)
+            const int j = jhi - w.lane; const bool act = j >= (int)L - 1;
             // `if (i<=1) break` (bwt.c:376): lanes below the first finished lane with i<=1 were never run by the reference
             const uint32_t brk = w.ballot(act && cur.st == KJ_ST_EXACT && cur.i <= 1);
             const int cut = brk ? kj_ffs(brk) - 1 : 31;
@@ -962,11 +922,11 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
                     if (round > 0 && !have_nxt && jhi - 32 >= 0) {
                         // (not before the first round: a full-length match ends the fragment with one chain.)  The lowest open chain
                         // has no ended chain below it in this block: fetch the bound from the next block's phase A
-                        const uint32_t inf = w.ballot(probe && cur.st != KJ_ST_OPEN);
+                        const uint32_t inf = w.ballot(act && cur.st != KJ_ST_OPEN);
                         if ((31 - kj_clz(om)) > (inf ? 31 - kj_clz(inf) : -1)) { jstart = jhi - 32; start_la = true; continue; }
                     }
                     if (have_nxt) lb_ext = kj_block_lb_ext<IdxT>(w, nxt, jhi - 32 - w.lane >= 0, jhi - 32 - w.lane, kk);
-                    lb = kj_chain_lb<IdxT>(w, cur, probe, j, kk, lb_ext);
+                    lb = kj_chain_lb<IdxT>(w, cur, act, j, kk, lb_ext);
                 }
                 // L as the reference holds it when it reaches lane x: the finished chains above x (the open ones above x are completed
                 // before x can be skipped for good: the test is repeated every round)
@@ -1089,10 +1049,8 @@ static KJ_DEV void kj_protein_fragments(KjWarpCtx& cx, KjQueue& q, const uint8_t
         aa[3 * t] = (u >= 'A' && u <= 'Z') ? tb.aa_index[u - 'A'] : (uint8_t)0;
     }
     w.sync();
-#ifndef KJ_SPLIT_UNROLLED_GREEDY
-    if (small_code) kj_split_frames_rolled(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1); else
-#endif
-    kj_split_frames(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
+    if (small_code) kj_split_frames_rolled(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
+    else kj_split_frames(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1158,24 +1116,7 @@ static KJ_DEV uint32_t kj_classify_item(KjWarpCtx& cx, const uint8_t* s1, int n1
             else kj_translate_pair(cx, q, s1, n1, n1 >= m3, s2, n2, paired && n2 >= m3, greedy, small_code);   // a short mate is skipped individually (699, 705)
         }
         if (ok && MODE == 1) kj_queue_sort(cx, q);     // greedy pops every fragment (and many variants): ranking once pays (A/B); MEM stops after a few pops (slower with it)
-        if (ROLE == 1) {
-            // The search would run the SEG gate on every fragment it pops; for most of them the window classes already say "nothing to mask" (kj_seg
-            // returns 0 and the fragment is searched as it is).  Decide that here, for every queued fragment, and mark it as checked: the class scan
-            // leaves the search kernel's hot loop (a few per cent of its instructions and of its hot code) for this kernel, which has issue slots to spare.
-#ifdef KJ_FRONT_SEG      // slower in an A/B run (front end not yet running beside the search): the scan of ALL queued fragments costs more than the popped ones save
-            if (ok && MODE == 1 && rp.seg) {
-                KJ_ROLLED
-                for (uint32_t i = 0; i < q.n; i++) {
-                    const uint32_t p = q.pay[i]; const uint32_t arr = p >> 30, start = (p >> 14) & 0x7fffu, len = p & 0x3fffu;
-                    bool clean = (int)len < KJ_SEG_WINDOW;
-                    if (!clean) { kj_load_frag(cx, arr, start, len); clean = !kj_seg_flags(cx, (int)len, false); }
-                    if (clean && cx.w.lane == 0) q.pay[i] = p | (1u << 29);
-                    cx.w.sync();
-                }
-            }
-#endif
-            kj_prep_store(cx, q, ok, rec); return KJ_TAX_BAD;
-        }
+        if (ROLE == 1) { kj_prep_store(cx, q, ok, rec); return KJ_TAX_BAD; }
         if (!ok) return KJ_TAX_BAD;
     } else if (!kj_prep_load(cx, q, rec)) return KJ_TAX_BAD;
     double query_len;                                                    // E-value query length (659, 698, 704)

@@ -136,7 +136,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
 #if defined(KJ_EMU)
             const int i0_ = one.i;
 #endif
-            kj_chain_finish<IdxT, true>(ix, frag, one);                          // every lane runs the same chain: identical addresses, one sector per step
+            kj_chain_finish<IdxT>(ix, frag, one);                          // every lane runs the same chain: identical addresses, one sector per step
 #if defined(KJ_EMU)
             if (w.lane == 0) kj_emu_stats.var_steps += (unsigned long long)(i0_ - one.i + 1);
 #endif
@@ -159,20 +159,12 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             for (;;) {                                                             // same skeleton as kj_mem_item: one phase-A site, one completion site
                 if (jstart >= 0) {
                     KjChain<IdxT> t; t.lo = 0; t.hi = 0; t.i = 0; t.st = KJ_ST_EXACT;
-#ifndef KJ_PROBE
-                    if (jstart - w.lane >= L - 1 || (start_la && jstart - w.lane >= 0)) kj_chain_start<IdxT, true>(ix, frag, jstart - w.lane, rp.seed_length, t);
-#else
-                    if (jstart - w.lane >= 0) kj_chain_start<IdxT, true>(ix, frag, jstart - w.lane, rp.seed_length, t);
-#endif
+                    if (jstart - w.lane >= L - 1 || (start_la && jstart - w.lane >= 0)) kj_chain_start<IdxT>(ix, frag, jstart - w.lane, rp.seed_length, t);
                     w.sync();
                     if (start_la) { nxt = t; have_nxt = true; } else { cur = t; round = 0; }
                     jstart = -1;
                 }
-#ifndef KJ_PROBE
-                const int j = jhi - w.lane; const bool act = j >= L - 1; const bool probe = act;
-#else
-                const int j = jhi - w.lane; const bool probe = j >= 0; const bool act = j >= L - 1;
-#endif
+                const int j = jhi - w.lane; const bool act = j >= L - 1;
                 const uint32_t brk = w.ballot(act && cur.st == KJ_ST_EXACT && cur.i <= 1);        // `if (i<=1) break` (bwt.c:292)
                 const int cut = brk ? kj_ffs(brk) - 1 : 31;
                 const bool open = act && cur.st == KJ_ST_OPEN && w.lane <= cut;
@@ -183,11 +175,11 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                     if (mono) {
                         int lb_ext = 0;
                         if (round > 0 && !have_nxt && jhi - 32 >= 0) {
-                            const uint32_t inf = w.ballot(probe && cur.st != KJ_ST_OPEN);
+                            const uint32_t inf = w.ballot(act && cur.st != KJ_ST_OPEN);
                             if ((31 - kj_clz(om)) > (inf ? 31 - kj_clz(inf) : -1)) { jstart = jhi - 32; start_la = true; continue; }
                         }
                         if (have_nxt) lb_ext = kj_block_lb_ext<IdxT>(w, nxt, jhi - 32 - w.lane >= 0, jhi - 32 - w.lane, kk);
-                        lb = kj_chain_lb<IdxT>(w, cur, probe, j, kk, lb_ext);
+                        lb = kj_chain_lb<IdxT>(w, cur, act, j, kk, lb_ext);
                     }
                     // an open chain is not recorded if its match is shorter than L or cannot start left of a qualifying finished chain above it
                     const bool qual = act && cur.st == KJ_ST_EXACT && w.lane <= cut && j - cur.i + 1 >= L;
@@ -199,7 +191,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                     const bool top = need && !(w.lane > 0 && ((nm >> (w.lane - 1)) & 1u));
                     const int group = (round == 0 && mono) ? 0 : KJ_GROUP_LATE;
                     const bool sel = need && (top || kj_popc(nm & lanemask_lt(w.lane)) < group);
-                    kj_finish_selected<IdxT, true>(w, ix, frag, sel, cur);
+                    kj_finish_selected<IdxT>(w, ix, frag, sel, cur);
                     round++;
                     continue;
                 }
@@ -296,7 +288,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                         const uint32_t failmask = ~w.ballot(pass) & 0x7ffffu;
                         const int n_ok = failmask ? kj_ffs(failmask) - 1 : 19;      // first failing substitute ends the loop (391)
                         IdxT lo = (IdxT)sm.lo, hi = (IdxT)(sm.lo + sm.len); bool ok = false;
-                        if (w.lane < n_ok) ok = kj_update_si<IdxT, true>(ix, sub, lo, hi);
+                        if (w.lane < n_ok) ok = kj_update_si<IdxT>(ix, sub, lo, hi);
                         w.sync();
                         const uint32_t okmask = w.ballot(ok); const uint32_t cnt = (uint32_t)kj_popc(okmask);
                         if (cnt) {

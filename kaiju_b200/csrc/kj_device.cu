@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -23,16 +24,10 @@
 #include "kj_host.h"
 
 #define KJ_WARPS_PER_CTA 8
-#ifndef KJ_MIN_BLOCKS
 #define KJ_MIN_BLOCKS 4          // resident CTAs per SM the register allocation is tuned for (the search is latency-bound; on an H100 (400 W) 4 beat 3 CTAs, 50.6 vs 46.5 M pairs/s MEM)
-#endif
-#ifndef KJ_MIN_BLOCKS_GREEDY_SPLIT
 #define KJ_MIN_BLOCKS_GREEDY_SPLIT 4   // front-end / search kernels of the two-kernel Greedy path: on an H100 (400 W) 4 CTAs (64 registers) beat 5 (48), 13.8 vs 12.9 M pairs/s
-#endif
-#ifndef KJ_MIN_BLOCKS_GREEDY
 #define KJ_MIN_BLOCKS_GREEDY 4   // 5 CTAs (48 registers) was slower in an A/B run: more warps, but more spill traffic and more instruction-fetch stalls
-#endif
-#define KJ_KEPT_SMEM_FIXED 20      // = KJ_KEPT_SMEM of kj_host.cpp (checked at launch: the fixed profile is only used when the layouts agree)
+#define KJ_CLAIM 4               // read items claimed per atomic by a warp
 #define KJ_CHUNK_READS (1u << 20)
 #define KJ_CHUNK_BYTES (1ull << 28)  // and at most this many bases of one mate per chunk (long reads)
 
@@ -40,32 +35,12 @@
 
 struct KjCtaShared { KjDevIndex ix; KjTables tb; };
 
-// ---- bulk copy (the Hopper copy engine, "TMA" in its 1-D form) of a warp's claimed reads into shared memory: one elected lane
-// arms the warp's mbarrier with the byte count and issues cp.async.bulk; the 32 lanes wait on the barrier's phase.  The translation
-// passes then read the bases from shared memory instead of waiting on global loads pass by pass.
-static __device__ __forceinline__ uint32_t kj_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-static __device__ __forceinline__ void kj_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(kj_smem_u32(bar)), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-static __device__ __forceinline__ void kj_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(kj_smem_u32(bar)), "r"(bytes) : "memory");
-}
-static __device__ __forceinline__ void kj_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(kj_smem_u32(dst)), "l"(src), "r"(bytes), "r"(kj_smem_u32(bar)) : "memory");
-}
-static __device__ __forceinline__ void kj_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile("{\n .reg .pred p;\n KJ_WAIT:\n mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n @p bra KJ_DONE;\n bra KJ_WAIT;\n KJ_DONE:\n}"
-                 :: "r"(kj_smem_u32(bar)), "r"(parity) : "memory");
-}
-
 // GWS = false: the per-warp work space is carved out of shared memory (the compiler keeps every access in the shared
 // address space); GWS = true (reads too long for that): the same carve-up in a global buffer, generic loads and stores.
 // FIX = true: the work-space carve-up of the standard short-read case (mates up to 152 bases, -m 11) as compile-time constants: every offset
 // becomes an immediate of the shared-memory instructions instead of a value that is kept in (or re-derived into) registers.
 static __host__ __device__ __forceinline__ KjRunParams kj_fixed_profile(int mode) {
-    KjRunParams p{}; p.mode = mode; p.m = 11; p.max_len = 152; p.max_frag = 152 / 3 + 1; p.item_cap = 128; p.kept_cap_smem = KJ_KEPT_SMEM_FIXED; p.stage = 0;
+    KjRunParams p{}; p.mode = mode; p.m = 11; p.max_len = 152; p.max_frag = 152 / 3 + 1; p.item_cap = 128; p.kept_cap_smem = KJ_KEPT_SMEM;
     return p;
 }
 // VB = true: the verbose outputs (id sets, accession sets, fragment strings) are compiled in; the kernels of the normal path carry none of it.
@@ -107,13 +82,6 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
     cx.gscratch = gscratch + gwarp * gscratch_bytes;
     cx.err = err; cx.text = nullptr; cx.text_cap = frag_stride; cx.text_len = 0; cx.want_acc = VB && acc_out != nullptr;
     const bool paired = seq2 != nullptr;
-#ifdef KJ_STAGE
-    const bool stage = !GWS && rp.stage != 0;
-#else
-    const bool stage = false;          // slower in an A/B run: the larger shared-memory carve-out shrinks the L1 that serves the rank loads
-#endif
-    uint64_t* mbar = (uint64_t*)(cx.smem + cx.L.mbar_off); uint8_t* stg = cx.smem + cx.L.stage_off; uint32_t phase = 0;
-    if (stage) { if (cx.w.lane == 0) kj_mbar_init(mbar, 1); cx.w.sync(); }
     // work distribution: a warp claims KJ_CLAIM consecutive items per atomic and fetches their offsets with one coalesced load
     KJ_ROLLED
     for (;;) {
@@ -124,28 +92,13 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
         const unsigned long long ri = r0 + (unsigned long long)cx.w.lane;
         uint64_t o1 = 0, o2 = 0;
         if (cx.w.lane <= KJ_CLAIM && ri <= n_reads) { o1 = off1[ri] - base1; if (paired) o2 = off2[ri] - base2; }
-        uint32_t al1 = 0, al2 = 0; uint64_t f1 = 0, f2 = 0;
-        if (stage) {
-            // the claimed reads are contiguous in the packed arrays: one bulk copy per mate, source and size rounded to 16 bytes
-            const int nk = (int)(n_reads - r0 < (unsigned long long)KJ_CLAIM ? n_reads - r0 : (unsigned long long)KJ_CLAIM);
-            f1 = cx.w.shfl64(o1, 0); f2 = cx.w.shfl64(o2, 0);
-            const uint64_t l1 = cx.w.shfl64(o1, nk), l2 = cx.w.shfl64(o2, nk);
-            al1 = (uint32_t)((uintptr_t)(seq1 + f1) & 15u); al2 = paired ? (uint32_t)((uintptr_t)(seq2 + f2) & 15u) : 0u;
-            const uint32_t b1 = (al1 + (uint32_t)(l1 - f1) + 15u) & ~15u, b2 = paired ? (al2 + (uint32_t)(l2 - f2) + 15u) & ~15u : 0u;
-            if (cx.w.lane == 0) {
-                kj_mbar_expect_tx(mbar, b1 + b2);
-                if (b1) kj_bulk_g2s(stg, seq1 + f1 - al1, b1, mbar);
-                if (b2) kj_bulk_g2s(stg + cx.L.stage_stride, seq2 + f2 - al2, b2, mbar);
-            }
-            kj_mbar_wait(mbar, phase); phase ^= 1u;
-        }
         KJ_ROLLED
         for (int k = 0; k < KJ_CLAIM; k++) {
             const unsigned long long r = r0 + (unsigned long long)k;
             if (r >= n_reads) break;
             const uint64_t a0 = cx.w.shfl64(o1, k), a1 = cx.w.shfl64(o1, k + 1), b0 = cx.w.shfl64(o2, k), b1 = cx.w.shfl64(o2, k + 1);
-            const uint8_t* p1 = stage ? stg + al1 + (uint32_t)(a0 - f1) : seq1 + a0;
-            const uint8_t* p2 = !paired ? nullptr : stage ? stg + cx.L.stage_stride + al2 + (uint32_t)(b0 - f2) : seq2 + b0;
+            const uint8_t* p1 = seq1 + a0;
+            const uint8_t* p2 = paired ? seq2 + b0 : nullptr;
             uint32_t best = 0;
             if (VB && frag_out) { cx.text = frag_out + r * frag_stride; cx.text_len = 0; }
             uint32_t t = kj_classify_item<MODE, IdxT, ROLE>(cx, p1, (int)(a1 - a0), p2, (int)(b1 - b0), paired, best, ROLE ? prep + (size_t)(r - r_begin) * prep_stride : nullptr);
@@ -182,6 +135,24 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
             cx.w.sync();
         }
     }
+}
+
+// Every instantiation has the same signature: the host picks one per launch (kj_select_kernel), sets it up and launches it through the pointer.
+using KjKernel = decltype(&kj_classify_kernel<0, uint32_t, false, false, false, 0>);
+// The fixed profile and the two-kernel pair exist for Greedy only (kj_use_fixed, launch()); neither applies to the verbose kernels or to a work space in global memory.
+template <int MODE, class T>
+static KjKernel kj_select_kernel_t(bool gws, bool fixed, bool verbose, int role) {
+    if (verbose) return gws ? kj_classify_kernel<MODE, T, true, false, true, 0> : kj_classify_kernel<MODE, T, false, false, true, 0>;
+    if (gws) return kj_classify_kernel<MODE, T, true, false, false, 0>;
+    if constexpr (MODE == 1) {
+        if (fixed) return role == 1 ? kj_classify_kernel<1, T, false, true, false, 1> : role == 2 ? kj_classify_kernel<1, T, false, true, false, 2> : kj_classify_kernel<1, T, false, true, false, 0>;
+        if (role) return role == 1 ? kj_classify_kernel<1, T, false, false, false, 1> : kj_classify_kernel<1, T, false, false, false, 2>;
+    }
+    return kj_classify_kernel<MODE, T, false, false, false, 0>;
+}
+static KjKernel kj_select_kernel(int mode, bool wide, bool gws, bool fixed, bool verbose, int role) {
+    if (mode == 0) return wide ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
+    return wide ? kj_select_kernel_t<1, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<1, uint32_t>(gws, fixed, verbose, role);
 }
 
 __global__ void kj_maxlen_kernel(const uint64_t* __restrict__ off, uint64_t n, unsigned int* __restrict__ out) {
@@ -241,7 +212,7 @@ struct kj_ctx {
     uint64_t* d_ids[2] = {nullptr, nullptr}; uint8_t* d_nids[2] = {nullptr, nullptr}; size_t d_ids_cap = 0;
     size_t d_reads_cap = 0;
     uint64_t launches = 0; double last_kernel_ms = 0.0;
-    int grid = 0; size_t smem_bytes = 0; int cfg_mode = -1;
+    int grid = 0; size_t smem_bytes = 0; KjKernel grid_kernel = nullptr;      // the last launch's geometry, and the kernel whose occupancy gave the grid
 };
 
 template <class T> static int upload(const std::vector<T>& v, void** d, uint64_t& total) {
@@ -257,52 +228,28 @@ template <class T> static int upload(const std::vector<T>& v, void** d, uint64_t
 #define KJ_SMEM_WS_LIMIT (75u * 1024u)
 // the fixed-profile kernels apply when the batch's carve-up is exactly the compiled-in one
 static bool kj_use_fixed(const KjRunParams& rp) {
-    if (rp.ws_global || rp.mode != 1 || getenv("KJ_NO_FIXED")) return false;      // A/B: faster for Greedy, slightly slower for MEM: Greedy only
+    if (rp.ws_global || rp.mode != 1) return false;      // Greedy only: faster for Greedy in an A/B run, slightly slower for MEM
     const KjSmemLayout a = kj_smem_layout(rp), b = kj_smem_layout(kj_fixed_profile(rp.mode));
-    return memcmp(&a, &b, sizeof a) == 0 && rp.max_len == 152 && rp.kept_cap_smem == KJ_KEPT_SMEM_FIXED;
+    return memcmp(&a, &b, sizeof a) == 0 && rp.max_len == 152 && rp.kept_cap_smem == KJ_KEPT_SMEM;
 }
-static int configure_launch(kj_ctx* c, KjRunParams& rp, size_t& smem, int& grid, bool verbose) {
-#ifdef KJ_STAGE
-    rp.stage = getenv("KJ_NO_STAGE") ? 0u : 1u;            // build with -DKJ_STAGE: bulk-copy staging of the bases (A/B; not the default, see the kernel)
-#else
-    rp.stage = 0u;
-#endif
-    KjSmemLayout L = kj_smem_layout(rp);
-    const size_t head = kj_align((uint32_t)sizeof(KjCtaShared), 16);
-    smem = head + (size_t)KJ_WARPS_PER_CTA * L.total;
-    size_t limit = KJ_SMEM_WS_LIMIT;
-    if (const char* v = getenv("KJ_WS_LIMIT_KB")) { long x = atol(v); if (x >= 0 && x <= 227) limit = (size_t)x * 1024u; }    // tuning hook (A/B of the switch point)
-    rp.ws_global = smem > limit ? 1u : 0u;
-    if (rp.ws_global) { smem = head; rp.stage = 0; }
-    const int cfg = rp.mode * 2 + (int)rp.ws_global + ((!verbose && kj_use_fixed(rp)) ? 4 : 0) + (verbose ? 8 : 0);
-    // The max-dynamic-shared-memory attribute belongs to the kernel instantiation on the device, not to a context: several contexts
-    // (or batches with different read lengths) share it, so it is only ever raised (process-wide table), never lowered.
-    static std::mutex attr_mu; static size_t attr_set[64][32];
-    const bool fixed = !verbose && kj_use_fixed(rp);
-    const int inst = rp.mode * 4 + (c->H.wide ? 2 : 0) + (int)rp.ws_global + (fixed ? 8 : 0) + (verbose ? 16 : 0);
-    bool raise = false;
-    { std::lock_guard<std::mutex> lk(attr_mu); if (c->device < 64 && smem > attr_set[c->device][inst]) { attr_set[c->device][inst] = smem; raise = true; } else if (c->device >= 64) raise = true; }
-    if (!raise && smem == c->smem_bytes && c->grid > 0 && c->cfg_mode == cfg) { grid = c->grid; return KJ_OK; }
-    int per_sm = 0;
-#define KJ_CFGR(M, T, G, F, V, R) { if (raise) CK(cudaFuncSetAttribute(kj_classify_kernel<M, T, G, F, V, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-                          CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kj_classify_kernel<M, T, G, F, V, R>, KJ_WARPS_PER_CTA * 32, smem)); }
-#define KJ_CFG(M, T, G, F, V) KJ_CFGR(M, T, G, F, V, 0)
-#define KJ_CFG2(M, T) { if (verbose) { if (rp.ws_global) KJ_CFG(M, T, true, false, true) else KJ_CFG(M, T, false, false, true) } \
-                        else if (rp.ws_global) KJ_CFG(M, T, true, false, false) else if (fixed) KJ_CFG(M, T, false, true, false) else KJ_CFG(M, T, false, false, false) }
-    // the Greedy front-end / search pair (launch()): the grid is the search kernel's, the front end needs no more than that
-#define KJ_CFGS(T) { if (fixed) { KJ_CFGR(1, T, false, true, false, 1) KJ_CFGR(1, T, false, true, false, 2) } else { KJ_CFGR(1, T, false, false, false, 1) KJ_CFGR(1, T, false, false, false, 2) } }
-    if (rp.mode == 0) { if (c->H.wide) KJ_CFG2(0, uint64_t) else KJ_CFG2(0, uint32_t) }
-    else {
-        if (c->H.wide) KJ_CFG2(1, uint64_t) else KJ_CFG2(1, uint32_t)
-        if (!rp.ws_global && !verbose && !getenv("KJ_NO_SPLIT")) { if (c->H.wide) KJ_CFGS(uint64_t) else KJ_CFGS(uint32_t) }
+// Prepares the kernels of one launch (`front` may be null) for `smem` bytes of dynamic shared memory and sets the persistent grid from the
+// occupancy of `kern`: with the Greedy front-end / search pair that is the search kernel, and the front end needs no more than that.
+static int configure_launch(kj_ctx* c, KjKernel front, KjKernel kern, size_t smem) {
+    {   // The max-dynamic-shared-memory attribute belongs to the kernel instantiation on the device, not to a context: several contexts
+        // (or batches with different read lengths) share it, so it is only ever raised (process-wide table), never lowered.
+        static std::mutex attr_mu; static std::map<std::pair<int, KjKernel>, size_t> attr_set;
+        std::lock_guard<std::mutex> lk(attr_mu);
+        for (KjKernel k : {front, kern}) {
+            if (!k) continue;
+            size_t& cur = attr_set[{c->device, k}];
+            if (smem > cur) { CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); cur = smem; }
+        }
     }
-#undef KJ_CFGS
-#undef KJ_CFG2
-#undef KJ_CFG
-#undef KJ_CFGR
-    c->cfg_mode = cfg;
+    if (kern == c->grid_kernel && smem == c->smem_bytes && c->grid > 0) return KJ_OK;
+    int per_sm = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, KJ_WARPS_PER_CTA * 32, smem));
     if (per_sm < 1) { kj_err() = "kernel does not fit on an SM"; return KJ_ERR_UNSUPPORTED; }
-    grid = c->sm_count * per_sm;             // persistent grid: a whole number of CTAs per SM
+    c->grid = c->sm_count * per_sm;          // persistent grid: a whole number of CTAs per SM
+    c->grid_kernel = kern; c->smem_bytes = smem;
     return KJ_OK;
 }
 
@@ -361,7 +308,7 @@ static int upload_descriptor(kj_ctx* c) {
     D.n_sa = c->n_sa; D.nseq = H.nseq;
     D.tax_parent = (const uint32_t*)c->d_tax_parent; D.tax_depth = (const uint32_t*)c->d_tax_depth; D.tax_id = (const uint64_t*)c->d_tax_id; D.n_tax = (uint32_t)H.tax_id.size();
     D.lnfact = (const double*)c->d_lnfact; D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? c->d_kmer : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = c->d_tables;
-    D.quirk_lo = H.quirk_lo; D.mono = (H.quirk_lo == ~0ull && !getenv("KJ_NOMONO")) ? 1 : 0; D.quirk_d = c->d_quirk;      // KJ_NOMONO: developer hook (A/B of the chain bounds)
+    D.quirk_lo = H.quirk_lo; D.mono = H.quirk_lo == ~0ull ? 1 : 0; D.quirk_d = c->d_quirk;
     if (!c->d_ix) CK(cudaMalloc((void**)&c->d_ix, sizeof(KjDevIndex)));
     CK(cudaMemcpy(c->d_ix, &D, sizeof(KjDevIndex), cudaMemcpyHostToDevice));
     if (c->d_kmer_mem && c->kmer_k_mem) {
@@ -518,15 +465,20 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     rp.ev_breaks = c->d_evbreaks; rp.n_ev_breaks = c->n_evbreaks;
     rp.variant_cap *= c->variant_boost;
     const bool verbose = d_ids || d_acc || d_frag;
-    size_t smem; int grid; int rc = configure_launch(c, rp, smem, grid, verbose); if (rc) return rc;
-    rc = ensure_scratch(c, slot, rp, grid); if (rc) return rc;
-    c->grid = grid; c->smem_bytes = smem;
-    if (time_it) CK(cudaEventRecord(c->ev_a, st));
     const KjSmemLayout lay = kj_smem_layout(rp);
+    const size_t head = kj_align((uint32_t)sizeof(KjCtaShared), 16), ws_smem = head + (size_t)KJ_WARPS_PER_CTA * lay.total;
+    rp.ws_global = ws_smem > KJ_SMEM_WS_LIMIT ? 1u : 0u;
+    const size_t smem = rp.ws_global ? head : ws_smem;
     const bool fixed = !verbose && kj_use_fixed(rp);
-    const KjDevIndex* dix = (rp.mode == 0 && c->d_ix_mem && rp.m >= (uint32_t)c->kmer_k_mem) ? c->d_ix_mem : c->d_ix;
     // Greedy with the work space in shared memory: front-end kernel + search kernel over sub-batches (the records of a sub-batch live in d_prep)
     const bool split = rp.mode == 1 && !rp.ws_global && !verbose && !getenv("KJ_NO_SPLIT");
+    const KjKernel kern = kj_select_kernel(rp.mode, c->H.wide, rp.ws_global, fixed, verbose, split ? 2 : 0);
+    const KjKernel front = split ? kj_select_kernel(rp.mode, c->H.wide, false, fixed, false, 1) : nullptr;
+    int rc = configure_launch(c, front, kern, smem); if (rc) return rc;
+    const int grid = c->grid;
+    rc = ensure_scratch(c, slot, rp, grid); if (rc) return rc;
+    if (time_it) CK(cudaEventRecord(c->ev_a, st));
+    const KjDevIndex* dix = (rp.mode == 0 && c->d_ix_mem && rp.m >= (uint32_t)c->kmer_k_mem) ? c->d_ix_mem : c->d_ix;
     const uint32_t pstride = split ? kj_prep_stride(rp) : 0u; uint64_t sub = n;
     if (split) {
         // records of one sub-batch per buffer; two buffers per slot (the front end of sub-batch b+1 runs in the tail of the search of sub-batch b).
@@ -545,48 +497,33 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
         if (const char* v = getenv("KJ_SPLIT_SUB")) { const long long x = atoll(v); if (x >= 1024 && (uint64_t)x < sub) sub = (uint64_t)x; }
         sub = std::min(sub, n);
     }
-#define KJ_ARGS(B0, B1) dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, (uint64_t)(B1), d_tax, d_best, d_ids, d_nids, d_compact, \
-            ctr, c->d_spill[slot], c->d_gscratch[slot], kj_greedy_scratch_bytes(rp), rp.ws_global ? c->d_ws[slot] : nullptr, d_count_dst, c->d_err, d_acc, d_nacc, d_frag, frag_stride, d_fraglen, pbuf, pstride, (uint64_t)(B0)
-#define KJ_LAUNCH3(M, T, G, F, V, R, B0, B1) kj_classify_kernel<M, T, G, F, V, R><<<kgrid, KJ_WARPS_PER_CTA * 32, smem, kst>>>(KJ_ARGS(B0, B1))
-#define KJ_LAUNCH(M, T) if (verbose) { if (rp.ws_global) KJ_LAUNCH3(M, T, true, false, true, 0, 0, n); else KJ_LAUNCH3(M, T, false, false, true, 0, 0, n); } \
-                        else if (rp.ws_global) KJ_LAUNCH3(M, T, true, false, false, 0, 0, n); else if (fixed) KJ_LAUNCH3(M, T, false, true, false, 0, 0, n); else KJ_LAUNCH3(M, T, false, false, false, 0, 0, n)
-#define KJ_LAUNCH_SPLIT(T, R, B0, B1) if (fixed) KJ_LAUNCH3(1, T, false, true, false, R, B0, B1); else KJ_LAUNCH3(1, T, false, false, false, R, B0, B1)
-    uint8_t* pbuf = nullptr; unsigned long long* ctr = c->d_counter + slot; cudaStream_t kst = st; int kgrid = grid;
-    // (A/B: a search grid that leaves one CTA slot per SM to the front end of the next sub-batch is slower -- 32 instead of 40 search warps per SM cost
-    // more than the hidden front end gives back; KJ_SPLIT_LEAVE_SLOT keeps the experiment)
-    const int per_sm = grid / c->sm_count; const int sgrid = (per_sm >= 3 && getenv("KJ_SPLIT_LEAVE_SLOT")) ? c->sm_count * (per_sm - 1) : grid;
+    // one kernel launch over items [b0, b1), claimed through the counter `ctr` (zeroed on the launch's stream first)
+    auto run = [&](KjKernel k, cudaStream_t s, unsigned long long* ctr, uint8_t* pbuf, uint64_t b0, uint64_t b1) -> int {
+        CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), s));
+        k<<<grid, KJ_WARPS_PER_CTA * 32, smem, s>>>(dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, b1, d_tax, d_best, d_ids, d_nids, d_compact,
+                                                     ctr, c->d_spill[slot], c->d_gscratch[slot], kj_greedy_scratch_bytes(rp), rp.ws_global ? c->d_ws[slot] : nullptr,
+                                                     d_count_dst, c->d_err, d_acc, d_nacc, d_frag, frag_stride, d_fraglen, pbuf, pstride, b0);
+        c->launches++;
+        return KJ_OK;
+    };
     if (split) {
-        // front end on the slot's own stream, search on the caller's: F(b) -> S(b) through ev_f, S(b) -> F(b+2) (same buffer) through ev_s
+        // front end on the slot's own stream, search on the caller's: F(b) -> S(b) through ev_f, S(b) -> F(b+2) (same buffer) through ev_s.
+        // (A search grid that leaves one CTA slot per SM to the front end of the next sub-batch was slower in an A/B run.)
         cudaStream_t fs = c->fstream[slot]; uint8_t* base = c->d_prep + (size_t)slot * (c->prep_bytes / 2); uint64_t k = 0;
         CK(cudaEventRecord(c->ev_in[slot], st)); CK(cudaStreamWaitEvent(fs, c->ev_in[slot], 0));      // the inputs may have been produced on the caller's stream
         for (uint64_t b0 = 0; b0 < n; b0 += sub, k++) {
             const uint64_t b1 = std::min(n, b0 + sub); const int pb = (int)(k & 1);
-            pbuf = base + (size_t)pb * (c->prep_bytes / 4);
+            uint8_t* pbuf = base + (size_t)pb * (c->prep_bytes / 4);
             CK(cudaStreamWaitEvent(fs, c->ev_s[slot][pb], 0));                 // the search that last read this buffer (of this or an earlier launch; no-op if none)
-            ctr = c->d_counter + 2 + slot; kst = fs; kgrid = grid;
-            CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), fs));
-            if (c->H.wide) KJ_LAUNCH_SPLIT(uint64_t, 1, b0, b1); else KJ_LAUNCH_SPLIT(uint32_t, 1, b0, b1);
+            if ((rc = run(front, fs, c->d_counter + 2 + slot, pbuf, b0, b1))) return rc;
             CK(cudaEventRecord(c->ev_f[slot][pb], fs));
-            ctr = c->d_counter + slot; kst = st; kgrid = sgrid;
             CK(cudaStreamWaitEvent(st, c->ev_f[slot][pb], 0));
-            CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), st));
-            if (c->H.wide) KJ_LAUNCH_SPLIT(uint64_t, 2, b0, b1); else KJ_LAUNCH_SPLIT(uint32_t, 2, b0, b1);
+            if ((rc = run(kern, st, c->d_counter + slot, pbuf, b0, b1))) return rc;
             CK(cudaEventRecord(c->ev_s[slot][pb], st));
-            c->launches += 2;
         }
-        c->launches--;          // (the common tail below counts one)
-    } else {
-        CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), st));
-        if (rp.mode == 0) { if (c->H.wide) KJ_LAUNCH(0, uint64_t); else KJ_LAUNCH(0, uint32_t); }
-        else { if (c->H.wide) KJ_LAUNCH(1, uint64_t); else KJ_LAUNCH(1, uint32_t); }
-    }
-#undef KJ_LAUNCH
-#undef KJ_LAUNCH3
-#undef KJ_LAUNCH_SPLIT
-#undef KJ_ARGS
+    } else if ((rc = run(kern, st, c->d_counter + slot, nullptr, 0, n))) return rc;
     CK(cudaGetLastError());
     if (time_it) CK(cudaEventRecord(c->ev_b, st));
-    c->launches++;
     return KJ_OK;
 }
 

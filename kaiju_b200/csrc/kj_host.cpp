@@ -408,10 +408,7 @@ void kj_fill_run_params(const kj_params& p, uint32_t max_len, KjRunParams& rp) {
     rp.max_frag = rp.max_len / 3 + 1;
     uint32_t per_class = (rp.max_frag + 1 + rp.m) / (rp.m + 1);
     rp.item_cap = 2 * 12 * per_class + 8; rp.item_cap = (rp.item_cap + 1) & ~1u;
-#ifndef KJ_KEPT_SMEM
-#define KJ_KEPT_SMEM 20
-#endif
-    rp.kept_cap_smem = KJ_KEPT_SMEM;       // = max_matches_SI (20): greedy keeps its best list here; 5 Greedy CTAs per SM fit with it
+    rp.kept_cap_smem = KJ_KEPT_SMEM;       // 5 Greedy CTAs per SM fit with it
     rp.scratch_entries = 4 * rp.max_len + 64;
     rp.variant_cap = rp.max_len <= 160 ? 256u : rp.max_len <= 512 ? 1024u : 4096u;    // entries of the Greedy variant ring (it grows x4 and the call is repeated if a read fills it)
     if (const char* v = getenv("KJ_VARIANT_CAP")) { long x = atol(v); if (x >= 32 && x <= (1 << 20)) rp.variant_cap = (uint32_t)x; }   // test hook: provoke the overflow/retry path

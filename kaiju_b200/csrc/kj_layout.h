@@ -37,6 +37,7 @@ static inline uint32_t kj_rank_words(int wide) { return wide ? KJ_RANK_WORDS_WID
 #define KJ_TAX_BAD 0xffffffffu     // "bad number" database name (ConsumerThread.cpp:817-820): skipped
 #define KJ_MAX_MM 8                // max supported -e
 #define KJ_SEG_WINDOW 12
+#define KJ_KEPT_SMEM 20            // winners kept in shared memory before spilling = max_matches_SI (20): greedy keeps its best list there
 
 // wide records: hdr = cnt (40 bit: C[c] + #c before the block) | popc(w0) << 40 | (popc(w0)+popc(w1)) << 48 ; w0..w2 = one-hot bitmap.
 #define KJ_CNT_MASK 0xffffffffffull
@@ -89,5 +90,4 @@ struct KjRunParams {
     uint32_t scratch_entries;       // global spill entries per warp
     uint32_t variant_cap;           // Greedy: entries of the per-warp substituted-variant ring
     uint32_t ws_global;             // 1: the per-warp work space lives in global memory (reads too long for shared memory)
-    uint32_t stage;                 // 1: the bases of the reads a warp has claimed are brought into shared memory with one bulk copy per mate (kj_device.cu)
 };
