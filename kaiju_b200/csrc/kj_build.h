@@ -182,17 +182,16 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
     KjBuildLcode lc; memcpy(lc.v, lcode, 256);
     const int grid_big = c->sm_count * 16;
     // ---- BWT bytes to the device (freed again below)
-    uint8_t* d_bwt = nullptr; CK(cudaMalloc((void**)&d_bwt, (size_t)v.bwtlen));
-    struct Free { void* p; ~Free() { if (p) cudaFree(p); } } free_bwt{d_bwt};
-    int rc = kj_bld_upload(d_bwt, v.bwt, (size_t)v.bwtlen); if (rc) return rc;
+    KjDevBuf bwt; int rc = bwt.grow((size_t)v.bwtlen); if (rc) return rc;
+    const uint8_t* d_bwt = bwt.as<uint8_t>();
+    if ((rc = kj_bld_upload(bwt.p, v.bwt, (size_t)v.bwtlen))) return rc;
     // ---- letter counts per tile, C[]
     const uint64_t ntiles = (nb + KJ_BLD_THREADS - 1) / KJ_BLD_THREADS;
     if (ntiles >= (1ull << 31)) { kj_err() = "index too large"; return KJ_ERR_UNSUPPORTED; }
-    uint32_t* d_tc = nullptr; uint64_t* d_tp = nullptr; uint64_t* d_small = nullptr;
-    CK(cudaMalloc((void**)&d_tc, ntiles * KJ_MAX_ALEN * 4)); Free f1{d_tc};
-    CK(cudaMalloc((void**)&d_tp, ntiles * KJ_MAX_ALEN * 8)); Free f2{d_tp};
-    CK(cudaMalloc((void**)&d_small, 3 * KJ_MAX_ALEN * 8 + 64)); Free f3{d_small};
-    uint64_t* d_tot = d_small; uint64_t* d_C = d_small + KJ_MAX_ALEN + 1;
+    KjDevBuf tc, tp, small;
+    if ((rc = tc.grow(ntiles * KJ_MAX_ALEN * 4)) || (rc = tp.grow(ntiles * KJ_MAX_ALEN * 8)) || (rc = small.grow(3 * KJ_MAX_ALEN * 8 + 64))) return rc;
+    uint32_t* d_tc = tc.as<uint32_t>(); uint64_t* d_tp = tp.as<uint64_t>();
+    uint64_t* d_tot = small.as<uint64_t>(); uint64_t* d_C = d_tot + KJ_MAX_ALEN + 1;
     if (wide) kj_bld_count<KJ_RANK_ROWS_WIDE><<<(unsigned)ntiles, KJ_BLD_THREADS>>>(d_bwt, lc, n, rep, alen, d_tc);
     else kj_bld_count<KJ_RANK_ROWS_NARROW><<<(unsigned)ntiles, KJ_BLD_THREADS>>>(d_bwt, lc, n, rep, alen, d_tc);
     kj_bld_scan_tiles<<<1, 32 * KJ_MAX_ALEN>>>(d_tc, ntiles, d_tp, d_tot);
@@ -203,48 +202,59 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
     CK(cudaMemcpy(d_C, H.C, sizeof(uint64_t) * (size_t)(alen + 1), cudaMemcpyHostToDevice));
     // ---- rank records
     const size_t rank_bytes = (size_t)alen * nb * RW * 8;
-    CK(cudaMalloc(&c->d_rank, rank_bytes)); tot += rank_bytes;
+    if ((rc = c->rank.grow(rank_bytes))) return rc;
+    tot += rank_bytes;
     {
         const size_t smem = (size_t)KJ_BLD_THREADS * (RB + 4) + 64;
         if (wide) {
             CK(cudaFuncSetAttribute(kj_bld_records<KJ_RANK_ROWS_WIDE, KJ_RANK_WORDS_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            kj_bld_records<KJ_RANK_ROWS_WIDE, KJ_RANK_WORDS_WIDE><<<(unsigned)ntiles, KJ_BLD_THREADS, smem>>>(d_bwt, lc, n, rep, alen, nb, d_tp, d_C, (uint64_t*)c->d_rank);
-        } else kj_bld_records<KJ_RANK_ROWS_NARROW, KJ_RANK_WORDS_NARROW><<<(unsigned)ntiles, KJ_BLD_THREADS, smem>>>(d_bwt, lc, n, rep, alen, nb, d_tp, d_C, (uint64_t*)c->d_rank);
+            kj_bld_records<KJ_RANK_ROWS_WIDE, KJ_RANK_WORDS_WIDE><<<(unsigned)ntiles, KJ_BLD_THREADS, smem>>>(d_bwt, lc, n, rep, alen, nb, d_tp, d_C, c->rank.as<uint64_t>());
+        } else kj_bld_records<KJ_RANK_ROWS_NARROW, KJ_RANK_WORDS_NARROW><<<(unsigned)ntiles, KJ_BLD_THREADS, smem>>>(d_bwt, lc, n, rep, alen, nb, d_tp, d_C, c->rank.as<uint64_t>());
         CK(cudaGetLastError());
     }
     // ---- packed letters
     const uint64_t nwords = n / KJ_LETTERS_PER_WORD + 2;
-    CK(cudaMalloc(&c->d_letters, nwords * 8)); tot += nwords * 8;
-    kj_bld_letters<<<grid_big, 256>>>(d_bwt, lc, n, rep, nwords, (uint64_t*)c->d_letters);
+    if ((rc = c->letters.grow(nwords * 8))) return rc;
+    tot += nwords * 8;
+    kj_bld_letters<<<grid_big, 256>>>(d_bwt, lc, n, rep, nwords, c->letters.as<uint64_t>());
     CK(cudaGetLastError()); CK(cudaDeviceSynchronize());
-    cudaFree(d_bwt); free_bwt.p = nullptr; cudaFree(d_tc); f1.p = nullptr; cudaFree(d_tp); f2.p = nullptr;
+    bwt.reset(); tc.reset(); tp.reset();      // before the suffix-array arrays are allocated
     c->launches += 4;
     // ---- sequence -> taxon, sampled suffix array -> taxon
-    { size_t b = std::max<size_t>(H.seq_tax.size() * 4, 16); CK(cudaMalloc(&c->d_seq_tax, b)); tot += b; if (!H.seq_tax.empty()) CK(cudaMemcpy(c->d_seq_tax, H.seq_tax.data(), H.seq_tax.size() * 4, cudaMemcpyHostToDevice)); }
-    if (!H.seq_acc.empty()) { CK(cudaMalloc(&c->d_seq_acc, H.seq_acc.size() * 4)); tot += H.seq_acc.size() * 4; CK(cudaMemcpy(c->d_seq_acc, H.seq_acc.data(), H.seq_acc.size() * 4, cudaMemcpyHostToDevice)); }
+    if ((rc = upload(H.seq_tax, c->seq_tax, tot))) return rc;
+    if (!H.seq_acc.empty()) {
+        if ((rc = c->seq_acc.grow(H.seq_acc.size() * 4))) return rc;
+        tot += H.seq_acc.size() * 4; CK(cudaMemcpy(c->seq_acc.p, H.seq_acc.data(), H.seq_acc.size() * 4, cudaMemcpyHostToDevice));
+    }
+    uint32_t* d_err = c->err.as<uint32_t>();
     uint64_t n_sa;
     if (rep == 1) {
         n_sa = (uint64_t)v.ncheck;
-        CK(cudaMalloc(&c->d_sa_tax, (n_sa + 1) * 4)); tot += (n_sa + 1) * 4;
-        CK(cudaMemset((uint32_t*)c->d_sa_tax + n_sa, 0xff, 4));       // guard entry (see create_ctx): the last sampled row has no entry in a reference-built index
-        if (c->d_seq_acc) { CK(cudaMalloc(&c->d_sa_acc, (n_sa + 1) * 4)); tot += (n_sa + 1) * 4; CK(cudaMemset((uint32_t*)c->d_sa_acc + n_sa, 0xff, 4)); }
+        if ((rc = c->sa_tax.grow((n_sa + 1) * 4))) return rc;
+        tot += (n_sa + 1) * 4;
+        CK(cudaMemset(c->sa_tax.as<uint32_t>() + n_sa, 0xff, 4));       // guard entry (see create_ctx): the last sampled row has no entry in a reference-built index
+        if (c->seq_acc.p) {
+            if ((rc = c->sa_acc.grow((n_sa + 1) * 4))) return rc;
+            tot += (n_sa + 1) * 4; CK(cudaMemset(c->sa_acc.as<uint32_t>() + n_sa, 0xff, 4));
+        }
         const uint64_t CHE = (uint64_t)1 << 26;                        // entries per upload chunk
-        uint8_t* d_sa = nullptr; CK(cudaMalloc((void**)&d_sa, (size_t)std::min<uint64_t>(CHE, std::max<uint64_t>(n_sa, 1)) * (size_t)v.nbytes)); Free f4{d_sa};
+        KjDevBuf sa; if ((rc = sa.grow((size_t)std::min<uint64_t>(CHE, std::max<uint64_t>(n_sa, 1)) * (size_t)v.nbytes))) return rc;
         for (uint64_t e0 = 0; e0 < n_sa; e0 += CHE) {
             const uint64_t m = std::min(CHE, n_sa - e0);
-            CK(cudaMemcpy(d_sa, v.sa + e0 * (uint64_t)v.nbytes, (size_t)m * (size_t)v.nbytes, cudaMemcpyHostToDevice));
-            kj_bld_sa_tax<<<grid_big, 256>>>(d_sa, m, e0, v.nbytes, v.pbits, (uint32_t)v.nseq, (const uint32_t*)c->d_seq_tax, (uint32_t*)c->d_sa_tax, c->d_err);
-            if (c->d_sa_acc) kj_bld_sa_tax<<<grid_big, 256>>>(d_sa, m, e0, v.nbytes, v.pbits, (uint32_t)v.nseq, (const uint32_t*)c->d_seq_acc, (uint32_t*)c->d_sa_acc, c->d_err);
+            CK(cudaMemcpy(sa.p, v.sa + e0 * (uint64_t)v.nbytes, (size_t)m * (size_t)v.nbytes, cudaMemcpyHostToDevice));
+            kj_bld_sa_tax<<<grid_big, 256>>>(sa.as<uint8_t>(), m, e0, v.nbytes, v.pbits, (uint32_t)v.nseq, c->seq_tax.as<uint32_t>(), c->sa_tax.as<uint32_t>(), d_err);
+            if (c->sa_acc.p) kj_bld_sa_tax<<<grid_big, 256>>>(sa.as<uint8_t>(), m, e0, v.nbytes, v.pbits, (uint32_t)v.nseq, c->seq_acc.as<uint32_t>(), c->sa_acc.as<uint32_t>(), d_err);
             CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches++;
         }
-        uint32_t e = 0; CK(cudaMemcpy(&e, c->d_err, 4, cudaMemcpyDeviceToHost));
-        if (e & 64u) { CK(cudaMemset(c->d_err, 0, 4)); kj_err() = "corrupt suffix array (sequence number out of range)"; return KJ_ERR_IO; }
+        uint32_t e = 0; CK(cudaMemcpy(&e, d_err, 4, cudaMemcpyDeviceToHost));
+        if (e & 64u) { CK(cudaMemset(d_err, 0, 4)); kj_err() = "corrupt suffix array (sequence number out of range)"; return KJ_ERR_IO; }
     } else {
         const int64_t last = (int64_t)((n - 1) >> H.sa_exp) - H.sa_bias;  // entry of the last sampled row
         n_sa = last >= 0 ? (uint64_t)last + 1 : 0;
-        CK(cudaMalloc(&c->d_sa_tax, std::max<size_t>(n_sa * 4, 16))); tot += std::max<size_t>(n_sa * 4, 16);
-        if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->d_ix, n_sa, H.sa_bias, H.sa_exp, n, rep, (uint32_t*)c->d_sa_tax);
-        else kj_bld_sa_tax_scaled<uint32_t><<<grid_big, 256>>>(base->d_ix, n_sa, H.sa_bias, H.sa_exp, n, rep, (uint32_t*)c->d_sa_tax);
+        if ((rc = c->sa_tax.grow(std::max<size_t>(n_sa * 4, 16)))) return rc;
+        tot += std::max<size_t>(n_sa * 4, 16);
+        if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        else kj_bld_sa_tax_scaled<uint32_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches++;
     }
     c->n_sa = n_sa;
@@ -252,37 +262,36 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
 }
 
 // quirk constants and the k-mer table need rank queries on the finished records: run after the device descriptor exists
-// d_dst/k_out: where the table and its k go (default: the context's table for both modes); the second, larger table of the MEM kernels passes its own
-static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, void** d_dst = nullptr, int* k_out = nullptr) {
-    KjHostIndex& H = c->H; const int wide = H.wide;
-    if (!d_dst) { d_dst = &c->d_kmer; k_out = &H.kmer_k; }
-    if (H.quirk_lo != ~0ull && d_dst == &c->d_kmer) {
-        if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(c->d_ix, H.bwtlen - 65536ull, c->d_quirk); else kj_bld_quirk<uint32_t><<<1, 32>>>(c->d_ix, H.bwtlen - 65536ull, c->d_quirk);
-        CK(cudaGetLastError()); CK(cudaMemcpy(H.quirk_d, c->d_quirk, sizeof H.quirk_d, cudaMemcpyDeviceToHost)); c->launches++;
+// dst/k_out: where the table and its k go (the context's table for both modes, or the second, larger table of the MEM kernels)
+static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, int& k_out) {
+    KjHostIndex& H = c->H; const int wide = H.wide; const KjDevIndex* ix = c->ix.as<KjDevIndex>();
+    if (H.quirk_lo != ~0ull && &dst == &c->kmer) {
+        if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>()); else kj_bld_quirk<uint32_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        CK(cudaGetLastError()); CK(cudaMemcpy(H.quirk_d, c->quirk.p, sizeof H.quirk_d, cudaMemcpyDeviceToHost)); c->launches++;
     }
-    *k_out = 0;
+    k_out = 0;
     if (k < 2 || k > 7 || H.alen != 21) return KJ_OK;
     uint64_t n_final = 1; for (int d = 0; d < k; d++) n_final *= 20;
     { size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));      // two level buffers + the final table next to the index: a smaller k when that does not fit
       while (k > 2 && (double)n_final * (2.0 * sizeof(KjKmer) + sizeof(KjKmer32)) > 0.8 * (double)fr) { k--; n_final /= 20; } }
-    KjKmer* d_a = nullptr; KjKmer* d_b = nullptr;
-    CK(cudaMalloc((void**)&d_a, n_final * sizeof(KjKmer))); struct Free { void* p; ~Free() { if (p) cudaFree(p); } } fa{d_a};
-    CK(cudaMalloc((void**)&d_b, n_final * sizeof(KjKmer))); Free fb{d_b};
-    std::vector<KjKmer> first(20); for (uint32_t a = 0; a < 20; a++) { first[a].lo = H.C[a + 1]; first[a].hi = H.C[a + 2]; }
-    CK(cudaMemcpy(d_a, first.data(), 20 * sizeof(KjKmer), cudaMemcpyHostToDevice));
+    KjDevBuf a, b; int rc;
+    if ((rc = a.grow(n_final * sizeof(KjKmer))) || (rc = b.grow(n_final * sizeof(KjKmer)))) return rc;
+    std::vector<KjKmer> first(20); for (uint32_t l = 0; l < 20; l++) { first[l].lo = H.C[l + 1]; first[l].hi = H.C[l + 2]; }
+    CK(cudaMemcpy(a.p, first.data(), 20 * sizeof(KjKmer), cudaMemcpyHostToDevice));
     uint64_t n_cur = 20;
     for (int d = 1; d < k; d++) {
         const unsigned g = (unsigned)std::min<uint64_t>((n_cur * 20 + 255) / 256, (uint64_t)c->sm_count * 32);
-        if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(c->d_ix, d_a, n_cur, d_b); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(c->d_ix, d_a, n_cur, d_b);
+        if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>()); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         CK(cudaGetLastError()); c->launches++;
-        std::swap(d_a, d_b); fa.p = d_a; fb.p = d_b; n_cur *= 20;
+        std::swap(a, b); n_cur *= 20;
     }
-    if (wide) { *d_dst = d_a; fa.p = nullptr; tot += n_final * sizeof(KjKmer); }
+    if (wide) { dst = std::move(a); tot += n_final * sizeof(KjKmer); }
     else {
-        CK(cudaMalloc(d_dst, n_final * sizeof(KjKmer32))); tot += n_final * sizeof(KjKmer32);
-        kj_bld_kmer_narrow<<<c->sm_count * 8, 256>>>(d_a, n_final, (KjKmer32*)*d_dst); CK(cudaGetLastError()); c->launches++;
+        if ((rc = dst.grow(n_final * sizeof(KjKmer32)))) return rc;
+        tot += n_final * sizeof(KjKmer32);
+        kj_bld_kmer_narrow<<<c->sm_count * 8, 256>>>(a.as<KjKmer>(), n_final, dst.as<KjKmer32>()); CK(cudaGetLastError()); c->launches++;
     }
     CK(cudaDeviceSynchronize());
-    *k_out = k;
+    k_out = k;
     return KJ_OK;
 }

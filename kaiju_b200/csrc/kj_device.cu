@@ -182,43 +182,77 @@ __global__ void kj_count_commit(unsigned long long* __restrict__ total, unsigned
 }
 
 // ------------------------------------------------------------------------------------------------
+// The owner of every device allocation of the library: move-only, freed by its destructor (or early by reset()).
+struct KjDevBuf {
+    void* p = nullptr; size_t cap = 0;
+    KjDevBuf() = default;
+    KjDevBuf(const KjDevBuf&) = delete; KjDevBuf& operator=(const KjDevBuf&) = delete;
+    KjDevBuf(KjDevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    KjDevBuf& operator=(KjDevBuf&& o) noexcept { if (this != &o) { reset(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; } return *this; }
+    ~KjDevBuf() { reset(); }
+    void reset() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    // room for `need` bytes: only when the capacity is smaller, the buffer is freed and `alloc` (>= need) bytes are allocated
+    int grow(size_t need, size_t alloc) {
+        if (need <= cap) return KJ_OK;
+        reset(); void* q = nullptr; CK(cudaMalloc(&q, alloc)); p = q; cap = alloc; return KJ_OK;
+    }
+    int grow(size_t need) { return grow(need, need); }
+    template <class T> T* as() const { return (T*)p; }
+};
+
+// One of the two pipeline slots (the chunks of kj_classify, the lanes of kj_classify_files): staging, outputs, scratch, streams.
+// Two slots may be in flight, and their launches may have different run parameters (kj_classify_files derives them from each batch's longest
+// read): each slot has its own scratch, sized and grown from that slot's launches alone.  Carving both slots out of one buffer at offsets
+// computed from the current launch's parameters would let a launch with a smaller per-warp size land inside the region the other slot's
+// kernel is still using.  A slot's buffers are only replaced when its own previous work is complete; the cudaFree of the old buffer also
+// waits for the other slot's kernels.
+// Within one slot, the front-end kernel of the two-kernel Greedy path (ROLE 1) runs beside the search kernel (ROLE 2) of the previous
+// sub-batch; it touches neither the spill entries nor the variant ring (translation, queue ranking and the record store only use the
+// shared-memory work space), and the split path never uses the global work space, so the two share the slot's scratch safely.
+struct KjSlot {
+    KjDevBuf seq[2], off[2];                                        // staging of kj_classify (host buffers), one per mate
+    KjDevBuf tax, best, ids, nids, acc, nacc, frag, fraglen;        // outputs of a chunk
+    KjDevBuf spill, gscratch, ws;                                   // per-warp global scratch: spill entries, Greedy variant ring, work space of long reads
+    cudaStream_t stream = nullptr, fstream = nullptr;               // the slot's stream, and the front-end stream of the two-kernel Greedy path
+    cudaEvent_t ev_in = nullptr, ev_f[2] = {nullptr, nullptr}, ev_s[2] = {nullptr, nullptr};     // hand-over events between the two
+};
+
 struct KjFilesState; static void kj_files_state_free(KjFilesState* S);      // kj_ingest.h
 struct kj_ctx {
-    KjFilesState* files = nullptr;   // buffers of kj_classify_files, kept between calls
+    std::unique_ptr<KjFilesState, void (*)(KjFilesState*)> files{nullptr, kj_files_state_free};   // buffers of kj_classify_files, kept between calls
     int device = 0; kj_params params{}; int sm_count = 0;
     KjHostIndex H;                 // big arrays are released after upload; small ones stay
     KjDevIndex dix{};              // host copy of the descriptor (device pointers inside)
-    KjDevIndex* d_ix = nullptr; KjTables* d_tables = nullptr;
-    KjDevIndex* d_ix_mem = nullptr; void* d_kmer_mem = nullptr; int kmer_k_mem = 0;      // the MEM kernels' own descriptor: same index, 7-mer table (kj_create)
-    void* d_rank = nullptr; void* d_letters = nullptr; void* d_sa_tax = nullptr; void* d_seq_tax = nullptr;
-    void* d_sa_acc = nullptr; void* d_seq_acc = nullptr;
-    uint32_t* d_acc[2] = {nullptr, nullptr}; uint8_t* d_nacc[2] = {nullptr, nullptr}; char* d_frag[2] = {nullptr, nullptr}; uint32_t* d_fraglen[2] = {nullptr, nullptr}; size_t d_v2_cap = 0, d_frag_stride = 0;
-    void* d_tax_parent = nullptr; void* d_tax_depth = nullptr; void* d_tax_id = nullptr; void* d_lnfact = nullptr; void* d_kmer = nullptr;
+    KjDevBuf ix, tables;
+    KjDevBuf ix_mem, kmer_mem; int kmer_k_mem = 0;      // the MEM kernels' own descriptor: same index, 7-mer table (kj_create)
+    KjDevBuf rank, letters, sa_tax, seq_tax, sa_acc, seq_acc, tax_parent, tax_depth, tax_id, lnfact, kmer;
     uint64_t index_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;
     // run state
-    unsigned long long* d_counter = nullptr; uint32_t* d_err = nullptr; unsigned int* d_maxlen = nullptr;
-    // per-warp global scratch, one allocation per pipeline slot (ensure_scratch): spill entries, Greedy variant ring, work space of long reads
-    KjKept* d_spill[2] = {nullptr, nullptr}; size_t spill_bytes[2] = {0, 0}; uint8_t* d_gscratch[2] = {nullptr, nullptr}; size_t gscratch_bytes_total[2] = {0, 0};
-    double* d_evbreaks = nullptr; uint32_t n_evbreaks = 0; uint64_t* d_quirk = nullptr;
-    unsigned long long* d_counts = nullptr; unsigned long long* d_counts_pending = nullptr; uint32_t n_counts = 0, n_present = 0;   // per-taxon read counts (+1 slot: unclassified)
+    KjDevBuf counter, err, maxlen, quirk;
+    KjDevBuf evbreaks; uint32_t n_evbreaks = 0;
+    KjDevBuf counts, counts_pending; uint32_t n_counts = 0, n_present = 0;   // per-taxon read counts (+1 slot: unclassified)
     uint32_t variant_boost = 1;    // Greedy variant-ring capacity multiplier, raised after an overflow (flag 4) so that a retry succeeds
-    uint8_t* d_ws[2] = {nullptr, nullptr}; size_t ws_bytes[2] = {0, 0};
-    uint8_t* d_prep = nullptr; size_t prep_bytes = 0;      // prepared-item records of the two-kernel Greedy path (two slots x two buffers)
-    cudaStream_t fstream[2] = {nullptr, nullptr}; cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_f[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}}, ev_s[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // front-end stream + hand-over events per slot
-    cudaStream_t stream[2] = {nullptr, nullptr}; cudaEvent_t ev_a = nullptr, ev_b = nullptr;
-    // staging for kj_classify (host buffers)
-    uint8_t* d_seq[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}}; size_t d_seq_cap[2][2] = {{0, 0}, {0, 0}};
-    uint64_t* d_off[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}}; uint64_t* d_tax[2] = {nullptr, nullptr}; uint32_t* d_best[2] = {nullptr, nullptr};
-    uint64_t* d_ids[2] = {nullptr, nullptr}; uint8_t* d_nids[2] = {nullptr, nullptr}; size_t d_ids_cap = 0;
-    size_t d_reads_cap = 0;
+    KjDevBuf prep;                 // prepared-item records of the two-kernel Greedy path (two slots x two buffers)
+    KjSlot slot[2];
+    cudaEvent_t ev_a = nullptr, ev_b = nullptr;
     uint64_t launches = 0; double last_kernel_ms = 0.0;
     int grid = 0; size_t smem_bytes = 0; KjKernel grid_kernel = nullptr;      // the last launch's geometry, and the kernel whose occupancy gave the grid
 };
 
-template <class T> static int upload(const std::vector<T>& v, void** d, uint64_t& total) {
+// Where a launch writes its results (null: not wanted).  launch() takes device arrays; classify_host takes the host arrays the chunks are
+// copied back to (`compact` stays a device array) and fills in the slot's device arrays per chunk.
+struct KjOut {
+    uint64_t* tax = nullptr; uint32_t* best = nullptr; uint32_t* compact = nullptr;
+    uint64_t* ids = nullptr; uint8_t* nids = nullptr;                       // match-id sets (kj_classify_verbose)
+    uint32_t* acc = nullptr; uint8_t* nacc = nullptr;                        // accession sets (kj_classify_verbose2)
+    char* frag = nullptr; uint32_t frag_stride = 0; uint32_t* fraglen = nullptr;   // fragment strings (kj_classify_verbose2)
+    unsigned long long* counts = nullptr;                                    // per-taxon counts (launch() only)
+};
+
+template <class T> static int upload(const std::vector<T>& v, KjDevBuf& d, uint64_t& total) {
     size_t bytes = std::max<size_t>(v.size() * sizeof(T), 16);
-    CK(cudaMalloc(d, bytes));
-    if (!v.empty()) CK(cudaMemcpy(*d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    int rc = d.grow(bytes); if (rc) return rc;
+    if (!v.empty()) CK(cudaMemcpy(d.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
     total += bytes; return KJ_OK;
 }
 
@@ -253,32 +287,13 @@ static int configure_launch(kj_ctx* c, KjKernel front, KjKernel kern, size_t sme
     return KJ_OK;
 }
 
-// Two pipeline slots may be in flight, and their launches may have different run parameters (kj_classify_files derives them from each
-// batch's longest read): each slot has its own allocations, sized and grown from that slot's launch alone.  Carving both slots out of one
-// buffer at offsets computed from the current launch's parameters would let a launch with a smaller per-warp size land inside the region
-// the other slot's kernel is still using.  A slot's buffers are only replaced when its own previous work is complete; the cudaFree of the
-// old buffer also waits for the other slot's kernels.
-// Within one slot, the front-end kernel of the two-kernel Greedy path (ROLE 1) runs beside the search kernel (ROLE 2) of the previous
-// sub-batch; it touches neither the spill entries nor the variant ring (translation, queue ranking and the record store only use the
-// shared-memory work space), and the split path never uses the global work space, so the two share the slot's scratch safely.
-static int ensure_scratch(kj_ctx* c, int slot, const KjRunParams& rp, int grid) {
-    const size_t warps = (size_t)grid * KJ_WARPS_PER_CTA;
-    const size_t need = warps * rp.scratch_entries * sizeof(KjKept);
-    if (need > c->spill_bytes[slot]) { if (c->d_spill[slot]) cudaFree(c->d_spill[slot]); c->d_spill[slot] = nullptr; c->spill_bytes[slot] = 0; CK(cudaMalloc((void**)&c->d_spill[slot], need)); c->spill_bytes[slot] = need; }
-    const size_t gneed = warps * (size_t)kj_greedy_scratch_bytes(rp);
-    if (gneed > c->gscratch_bytes_total[slot]) { if (c->d_gscratch[slot]) cudaFree(c->d_gscratch[slot]); c->d_gscratch[slot] = nullptr; c->gscratch_bytes_total[slot] = 0; CK(cudaMalloc((void**)&c->d_gscratch[slot], gneed)); c->gscratch_bytes_total[slot] = gneed; }
-    const size_t wneed = rp.ws_global ? warps * (size_t)kj_smem_layout(rp).total : 0;
-    if (wneed > c->ws_bytes[slot]) { if (c->d_ws[slot]) cudaFree(c->d_ws[slot]); c->d_ws[slot] = nullptr; c->ws_bytes[slot] = 0; CK(cudaMalloc((void**)&c->d_ws[slot], wneed)); c->ws_bytes[slot] = wneed; }
-    return KJ_OK;
-}
-
 // E-value gate: break points of the minimal passing score (kj_build_evalue_breaks), rebuilt when the parameters change
 static int upload_evalue_breaks(kj_ctx* c) {
-    if (c->d_evbreaks) { cudaFree(c->d_evbreaks); c->d_evbreaks = nullptr; } c->n_evbreaks = 0;
+    c->evbreaks.reset(); c->n_evbreaks = 0;
     std::vector<double> br; int rc = kj_build_evalue_breaks(c->params, c->H.db_length, br); if (rc) return rc;
     if (br.empty()) return KJ_OK;
-    CK(cudaMalloc((void**)&c->d_evbreaks, br.size() * sizeof(double)));
-    CK(cudaMemcpy(c->d_evbreaks, br.data(), br.size() * sizeof(double), cudaMemcpyHostToDevice));
+    if ((rc = c->evbreaks.grow(br.size() * sizeof(double)))) return rc;
+    CK(cudaMemcpy(c->evbreaks.p, br.data(), br.size() * sizeof(double), cudaMemcpyHostToDevice));
     c->n_evbreaks = (uint32_t)br.size();
     return KJ_OK;
 }
@@ -293,53 +308,56 @@ static int new_ctx(kj_ctx** out, int device, const kj_params* params) {
     kj_ctx* c = new kj_ctx(); c->device = device; c->params = *params;
     std::unique_ptr<kj_ctx, void (*)(kj_ctx*)> guard(c, kj_destroy);
     cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, device)); c->sm_count = prop.multiProcessorCount;
-    CK(cudaMalloc((void**)&c->d_err, sizeof(uint32_t))); CK(cudaMemset(c->d_err, 0, sizeof(uint32_t)));
-    CK(cudaMalloc((void**)&c->d_quirk, sizeof c->H.quirk_d)); CK(cudaMemset(c->d_quirk, 0, sizeof c->H.quirk_d));
+    if ((rc = c->err.grow(sizeof(uint32_t)))) return rc;
+    CK(cudaMemset(c->err.p, 0, sizeof(uint32_t)));
+    if ((rc = c->quirk.grow(sizeof c->H.quirk_d))) return rc;
+    CK(cudaMemset(c->quirk.p, 0, sizeof c->H.quirk_d));
     *out = guard.release(); return KJ_OK;
 }
 // device descriptor from the context's device arrays + meta data
 static int upload_descriptor(kj_ctx* c) {
     KjHostIndex& H = c->H; KjDevIndex& D = c->dix; memset(&D, 0, sizeof D);
-    D.rank = (const uint64_t*)c->d_rank; D.nb = H.nb; D.letters = (const uint64_t*)c->d_letters; D.bwtlen = H.bwtlen; D.alen = H.alen;
+    D.rank = c->rank.as<const uint64_t>(); D.nb = H.nb; D.letters = c->letters.as<const uint64_t>(); D.bwtlen = H.bwtlen; D.alen = H.alen;
     for (int a = 0; a <= H.alen; a++) D.C[a] = H.C[a];
     for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
-    D.sa_acc = (const uint32_t*)c->d_sa_acc; D.seq_acc = (const uint32_t*)c->d_seq_acc;
-    D.sa_tax = (const uint32_t*)c->d_sa_tax; D.seq_tax = (const uint32_t*)c->d_seq_tax; D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
+    D.sa_acc = c->sa_acc.as<const uint32_t>(); D.seq_acc = c->seq_acc.as<const uint32_t>();
+    D.sa_tax = c->sa_tax.as<const uint32_t>(); D.seq_tax = c->seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
     D.n_sa = c->n_sa; D.nseq = H.nseq;
-    D.tax_parent = (const uint32_t*)c->d_tax_parent; D.tax_depth = (const uint32_t*)c->d_tax_depth; D.tax_id = (const uint64_t*)c->d_tax_id; D.n_tax = (uint32_t)H.tax_id.size();
-    D.lnfact = (const double*)c->d_lnfact; D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? c->d_kmer : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = c->d_tables;
-    D.quirk_lo = H.quirk_lo; D.mono = H.quirk_lo == ~0ull ? 1 : 0; D.quirk_d = c->d_quirk;
-    if (!c->d_ix) CK(cudaMalloc((void**)&c->d_ix, sizeof(KjDevIndex)));
-    CK(cudaMemcpy(c->d_ix, &D, sizeof(KjDevIndex), cudaMemcpyHostToDevice));
-    if (c->d_kmer_mem && c->kmer_k_mem) {
-        KjDevIndex M = D; M.kmer = c->d_kmer_mem; M.kmer_k = c->kmer_k_mem;
-        if (!c->d_ix_mem) CK(cudaMalloc((void**)&c->d_ix_mem, sizeof(KjDevIndex)));
-        CK(cudaMemcpy(c->d_ix_mem, &M, sizeof(KjDevIndex), cudaMemcpyHostToDevice));
+    D.tax_parent = c->tax_parent.as<const uint32_t>(); D.tax_depth = c->tax_depth.as<const uint32_t>(); D.tax_id = c->tax_id.as<const uint64_t>(); D.n_tax = (uint32_t)H.tax_id.size();
+    D.lnfact = c->lnfact.as<const double>(); D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? c->kmer.p : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = c->tables.as<KjTables>();
+    D.quirk_lo = H.quirk_lo; D.mono = H.quirk_lo == ~0ull ? 1 : 0; D.quirk_d = c->quirk.as<uint64_t>();
+    int rc = c->ix.grow(sizeof(KjDevIndex)); if (rc) return rc;
+    CK(cudaMemcpy(c->ix.p, &D, sizeof(KjDevIndex), cudaMemcpyHostToDevice));
+    if (c->kmer_mem.p && c->kmer_k_mem) {
+        KjDevIndex M = D; M.kmer = c->kmer_mem.p; M.kmer_k = c->kmer_k_mem;
+        if ((rc = c->ix_mem.grow(sizeof(KjDevIndex)))) return rc;
+        CK(cudaMemcpy(c->ix_mem.p, &M, sizeof(KjDevIndex), cudaMemcpyHostToDevice));
     }
     return KJ_OK;
 }
 static int upload_small(kj_ctx* c, uint64_t& tot) {
     KjHostIndex& H = c->H; int rc;
-    if ((rc = upload(H.tax_parent, &c->d_tax_parent, tot)) || (rc = upload(H.tax_depth, &c->d_tax_depth, tot)) || (rc = upload(H.tax_id, &c->d_tax_id, tot)) || (rc = upload(H.lnfact, &c->d_lnfact, tot))) return rc;
-    CK(cudaMalloc((void**)&c->d_tables, sizeof(KjTables))); CK(cudaMemcpy(c->d_tables, &H.tables, sizeof(KjTables), cudaMemcpyHostToDevice));
+    if ((rc = upload(H.tax_parent, c->tax_parent, tot)) || (rc = upload(H.tax_depth, c->tax_depth, tot)) || (rc = upload(H.tax_id, c->tax_id, tot)) || (rc = upload(H.lnfact, c->lnfact, tot)) ||
+        (rc = c->tables.grow(sizeof(KjTables)))) return rc;
+    CK(cudaMemcpy(c->tables.p, &H.tables, sizeof(KjTables), cudaMemcpyHostToDevice));
     return KJ_OK;
 }
 static int finish_ctx(kj_ctx* c, uint64_t tot) {
     KjHostIndex& H = c->H; int rc;
-    CK(cudaMemcpy(c->d_quirk, H.quirk_d, sizeof H.quirk_d, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->quirk.p, H.quirk_d, sizeof H.quirk_d, cudaMemcpyHostToDevice));
     if ((rc = upload_descriptor(c))) return rc;
     c->index_bytes = tot;
-    CK(cudaMalloc((void**)&c->d_counter, 4 * sizeof(unsigned long long))); CK(cudaMalloc((void**)&c->d_maxlen, 2 * sizeof(unsigned int)));       // counters: [slot] classify / search, [2 + slot] front end
-    for (int s = 0; s < 2; s++) {
-        CK(cudaStreamCreateWithFlags(&c->stream[s], cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&c->fstream[s], cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&c->ev_in[s], cudaEventDisableTiming));
-        for (int b = 0; b < 2; b++) { CK(cudaEventCreateWithFlags(&c->ev_f[s][b], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&c->ev_s[s][b], cudaEventDisableTiming)); }
+    if ((rc = c->counter.grow(4 * sizeof(unsigned long long))) || (rc = c->maxlen.grow(2 * sizeof(unsigned int)))) return rc;       // counters: [slot] classify / search, [2 + slot] front end
+    for (KjSlot& S : c->slot) {
+        CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&S.fstream, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&S.ev_in, cudaEventDisableTiming));
+        for (int b = 0; b < 2; b++) { CK(cudaEventCreateWithFlags(&S.ev_f[b], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&S.ev_s[b], cudaEventDisableTiming)); }
     }
     CK(cudaEventCreate(&c->ev_a)); CK(cudaEventCreate(&c->ev_b));
     if ((rc = upload_evalue_breaks(c))) return rc;
     c->n_counts = (uint32_t)H.tax_id.size() + 1u; c->n_present = H.n_present;
-    CK(cudaMalloc((void**)&c->d_counts, (size_t)c->n_counts * 8)); CK(cudaMalloc((void**)&c->d_counts_pending, (size_t)c->n_counts * 8));
-    CK(cudaMemset(c->d_counts, 0, (size_t)c->n_counts * 8)); CK(cudaMemset(c->d_counts_pending, 0, (size_t)c->n_counts * 8));
+    if ((rc = c->counts.grow((size_t)c->n_counts * 8)) || (rc = c->counts_pending.grow((size_t)c->n_counts * 8))) return rc;
+    CK(cudaMemset(c->counts.p, 0, (size_t)c->n_counts * 8)); CK(cudaMemset(c->counts_pending.p, 0, (size_t)c->n_counts * 8));
     return KJ_OK;
 }
 
@@ -352,9 +370,9 @@ template <class Fill> static int create_ctx(kj_ctx** out, int device, const kj_p
     // one guard entry: the reference's header counts one sampled row less than kaiju-mkbwt writes (suffixArray.c:160 vs 206-216), so the last
     // sampled row of an index has no entry; the reference reads past its array there, the device reads "no taxon"
     c->n_sa = H.sa_tax.size(); H.sa_tax.push_back(KJ_TAX_BAD);
-    if (!H.seq_acc.empty()) { H.sa_acc.push_back(0xffffffffu); if ((rc = upload(H.sa_acc, &c->d_sa_acc, tot)) || (rc = upload(H.seq_acc, &c->d_seq_acc, tot))) return rc; }
-    if ((rc = upload(H.rank, &c->d_rank, tot)) || (rc = upload(H.letters, &c->d_letters, tot)) || (rc = upload(H.sa_tax, &c->d_sa_tax, tot)) ||
-        (rc = upload(H.seq_tax, &c->d_seq_tax, tot)) || (rc = upload_small(c, tot)) || (rc = (H.wide ? upload(H.kmer, &c->d_kmer, tot) : upload(H.kmer32, &c->d_kmer, tot)))) return rc;
+    if (!H.seq_acc.empty()) { H.sa_acc.push_back(0xffffffffu); if ((rc = upload(H.sa_acc, c->sa_acc, tot)) || (rc = upload(H.seq_acc, c->seq_acc, tot))) return rc; }
+    if ((rc = upload(H.rank, c->rank, tot)) || (rc = upload(H.letters, c->letters, tot)) || (rc = upload(H.sa_tax, c->sa_tax, tot)) ||
+        (rc = upload(H.seq_tax, c->seq_tax, tot)) || (rc = upload_small(c, tot)) || (rc = (H.wide ? upload(H.kmer, c->kmer, tot) : upload(H.kmer32, c->kmer, tot)))) return rc;
     // host copies of the big arrays are no longer needed
     std::vector<uint64_t>().swap(H.rank); std::vector<uint64_t>().swap(H.letters); std::vector<uint32_t>().swap(H.sa_tax); std::vector<KjKmer>().swap(H.kmer); std::vector<KjKmer32>().swap(H.kmer32);
     if ((rc = finish_ctx(c, tot))) return rc;
@@ -372,13 +390,13 @@ static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, 
     if ((rc = upload_small(c, tot)) || (rc = kj_device_build(c, v, lcode, copies, base, tot))) return rc;
     c->H.kmer_k = 0;
     if ((rc = upload_descriptor(c))) return rc;
-    { const char* ek = getenv("KJ_KMER_K"); if ((rc = kj_device_build_kmer(c, ek ? atoi(ek) : kj_default_kmer_k(c->H.bwtlen), tot))) return rc; }
+    { const char* ek = getenv("KJ_KMER_K"); if ((rc = kj_device_build_kmer(c, ek ? atoi(ek) : kj_default_kmer_k(c->H.bwtlen), tot, c->kmer, c->H.kmer_k))) return rc; }
     // MEM runs faster with the intervals of all 20^7 7-mers (10.2 GB below 2^32 rows): one look-up replaces the first LF step of every chain, the one
     // with all 32 lanes alive.  Greedy loses with it (its seeds rarely get that far), so it keeps the 6-mer table: two descriptors, one index.
     // Only where HBM is plentiful: narrow indexes, and the two level buffers of the construction (41 GB) must fit next to the index.
     if (!c->H.wide && c->H.kmer_k == 6 && !kj_transient_ctx && !getenv("KJ_KMER_K") && !getenv("KJ_NO_KMER7")) {
         size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));
-        if ((double)fr > 1.28e9 * (2.0 * sizeof(KjKmer) + sizeof(KjKmer32)) + 16e9 && (rc = kj_device_build_kmer(c, 7, tot, &c->d_kmer_mem, &c->kmer_k_mem))) return rc;
+        if ((double)fr > 1.28e9 * (2.0 * sizeof(KjKmer) + sizeof(KjKmer32)) + 16e9 && (rc = kj_device_build_kmer(c, 7, tot, c->kmer_mem, c->kmer_k_mem))) return rc;
     }
     std::vector<uint32_t>().swap(c->H.seq_tax);
     if ((rc = finish_ctx(c, tot))) return rc;
@@ -408,7 +426,7 @@ extern "C" int kj_debug_index_checksums(kj_ctx* c, uint64_t out[8]) {
     const KjHostIndex& H = c->H; memset(out, 0, 64);
     const size_t sz[5] = {(size_t)H.alen * H.nb * kj_rank_words(H.wide) * 8, (size_t)(H.bwtlen / KJ_LETTERS_PER_WORD + 2) * 8, (size_t)c->n_sa * 4, (size_t)H.nseq * 4,
                           H.kmer_k ? (size_t)pow(20.0, H.kmer_k) * (H.wide ? sizeof(KjKmer) : sizeof(KjKmer32)) : 0};
-    const void* ptr[5] = {c->d_rank, c->d_letters, c->d_sa_tax, c->d_seq_tax, c->d_kmer};
+    const void* ptr[5] = {c->rank.p, c->letters.p, c->sa_tax.p, c->seq_tax.p, c->kmer.p};
     for (int i = 0; i < 5; i++) { std::vector<uint8_t> h(sz[i]); if (sz[i]) CK(cudaMemcpy(h.data(), ptr[i], sz[i], cudaMemcpyDeviceToHost)); out[i] = kj_mix_bytes(0x6b616a75ull + i, h.data(), h.size()); }
     out[5] = H.bwtlen; out[6] = (uint64_t)H.wide; out[7] = c->n_sa;
     return KJ_OK;
@@ -431,40 +449,31 @@ extern "C" int kj_set_params(kj_ctx* c, const kj_params* p) {
     CK(cudaSetDevice(c->device));
     c->params = *p;
     // the record buffers of the two-kernel Greedy path (up to 32 GB) go back when the context leaves Greedy mode
-    if (c->params.mode != 1 && c->d_prep) { CK(cudaDeviceSynchronize()); cudaFree(c->d_prep); c->d_prep = nullptr; c->prep_bytes = 0; }
+    if (c->params.mode != 1 && c->prep.p) { CK(cudaDeviceSynchronize()); c->prep.reset(); }
     return upload_evalue_breaks(c);
 }
 
 extern "C" void kj_destroy(kj_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    kj_files_state_free(c->files); c->files = nullptr;
-    if (c->d_ix_mem) cudaFree(c->d_ix_mem); if (c->d_kmer_mem) cudaFree(c->d_kmer_mem); if (c->d_prep) cudaFree(c->d_prep);
-    void* ptrs[] = {c->d_rank, c->d_letters, c->d_sa_tax, c->d_seq_tax, c->d_tax_parent, c->d_tax_depth, c->d_tax_id, c->d_lnfact, c->d_kmer, c->d_tables, c->d_ix,
-                    c->d_counter, c->d_err, c->d_maxlen, c->d_spill[0], c->d_spill[1], c->d_gscratch[0], c->d_gscratch[1], c->d_evbreaks, c->d_ws[0], c->d_ws[1], c->d_counts, c->d_counts_pending, c->d_quirk, c->d_tax[0], c->d_tax[1], c->d_best[0], c->d_best[1],
-                    c->d_seq[0][0], c->d_seq[0][1], c->d_seq[1][0], c->d_seq[1][1], c->d_off[0][0], c->d_off[0][1], c->d_off[1][0], c->d_off[1][1],
-                    c->d_ids[0], c->d_ids[1], c->d_nids[0], c->d_nids[1], c->d_sa_acc, c->d_seq_acc, c->d_acc[0], c->d_acc[1], c->d_nacc[0], c->d_nacc[1],
-                    c->d_frag[0], c->d_frag[1], c->d_fraglen[0], c->d_fraglen[1]};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    for (int s = 0; s < 2; s++) { if (c->stream[s]) cudaStreamDestroy(c->stream[s]); if (c->fstream[s]) cudaStreamDestroy(c->fstream[s]); if (c->ev_in[s]) cudaEventDestroy(c->ev_in[s]);
-                                  for (int b = 0; b < 2; b++) { if (c->ev_f[s][b]) cudaEventDestroy(c->ev_f[s][b]); if (c->ev_s[s][b]) cudaEventDestroy(c->ev_s[s][b]); } }
+    c->files.reset();      // first: it joins the parser thread
+    for (KjSlot& S : c->slot) { if (S.stream) cudaStreamDestroy(S.stream); if (S.fstream) cudaStreamDestroy(S.fstream); if (S.ev_in) cudaEventDestroy(S.ev_in);
+                               for (int b = 0; b < 2; b++) { if (S.ev_f[b]) cudaEventDestroy(S.ev_f[b]); if (S.ev_s[b]) cudaEventDestroy(S.ev_s[b]); } }
     if (c->ev_a) cudaEventDestroy(c->ev_a); if (c->ev_b) cudaEventDestroy(c->ev_b);
-    delete c;
+    delete c;              // the device buffers go with their owners
 }
 
 // one launch over reads [0,n) whose sequences/offsets are resident on the device
 static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_off1, const uint8_t* d_seq2, const uint64_t* d_off2, uint64_t base1, uint64_t base2,
-                  uint64_t n, uint32_t max1, uint32_t max2, uint64_t* d_tax, uint32_t* d_best, cudaStream_t st, bool time_it,
-                  uint64_t* d_ids = nullptr, uint8_t* d_nids = nullptr, unsigned long long* d_count_dst = nullptr, uint32_t* d_compact = nullptr,
-                  uint32_t* d_acc = nullptr, uint8_t* d_nacc = nullptr, char* d_frag = nullptr, uint32_t frag_stride = 0, uint32_t* d_fraglen = nullptr) {
+                  uint64_t n, uint32_t max1, uint32_t max2, const KjOut& o, cudaStream_t st, bool time_it) {
     if (c->params.input_is_protein) {
         if (d_seq2) { kj_err() = "protein input only supports one input (kaiju.cpp:201)"; return KJ_ERR_ARG; }
         if (max1 > KJ_MAX_PROTEIN_LEN) { kj_err() = "protein read longer than KJ_MAX_PROTEIN_LEN (5461 residues) is not supported"; return KJ_ERR_UNSUPPORTED; }
     } else if (max1 > KJ_MAX_READ_LEN || max2 > KJ_MAX_READ_LEN) { kj_err() = "read longer than KJ_MAX_READ_LEN (16383 bases) is not supported"; return KJ_ERR_UNSUPPORTED; }
     KjRunParams rp; kj_fill_run_params(c->params, std::max(max1, max2), rp);
-    rp.ev_breaks = c->d_evbreaks; rp.n_ev_breaks = c->n_evbreaks;
+    rp.ev_breaks = c->evbreaks.as<double>(); rp.n_ev_breaks = c->n_evbreaks;
     rp.variant_cap *= c->variant_boost;
-    const bool verbose = d_ids || d_acc || d_frag;
+    const bool verbose = o.ids || o.acc || o.frag;
     const KjSmemLayout lay = kj_smem_layout(rp);
     const size_t head = kj_align((uint32_t)sizeof(KjCtaShared), 16), ws_smem = head + (size_t)KJ_WARPS_PER_CTA * lay.total;
     rp.ws_global = ws_smem > KJ_SMEM_WS_LIMIT ? 1u : 0u;
@@ -476,22 +485,22 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     const KjKernel front = split ? kj_select_kernel(rp.mode, c->H.wide, false, fixed, false, 1) : nullptr;
     int rc = configure_launch(c, front, kern, smem); if (rc) return rc;
     const int grid = c->grid;
-    rc = ensure_scratch(c, slot, rp, grid); if (rc) return rc;
+    KjSlot& S = c->slot[slot];
+    const size_t warps = (size_t)grid * KJ_WARPS_PER_CTA;
+    if ((rc = S.spill.grow(warps * rp.scratch_entries * sizeof(KjKept))) || (rc = S.gscratch.grow(warps * (size_t)kj_greedy_scratch_bytes(rp))) ||
+        (rc = S.ws.grow(rp.ws_global ? warps * (size_t)lay.total : 0))) return rc;
     if (time_it) CK(cudaEventRecord(c->ev_a, st));
-    const KjDevIndex* dix = (rp.mode == 0 && c->d_ix_mem && rp.m >= (uint32_t)c->kmer_k_mem) ? c->d_ix_mem : c->d_ix;
+    const KjDevIndex* dix = (rp.mode == 0 && c->ix_mem.p && rp.m >= (uint32_t)c->kmer_k_mem) ? c->ix_mem.as<KjDevIndex>() : c->ix.as<KjDevIndex>();
     const uint32_t pstride = split ? kj_prep_stride(rp) : 0u; uint64_t sub = n;
     if (split) {
         // records of one sub-batch per buffer; two buffers per slot (the front end of sub-batch b+1 runs in the tail of the search of sub-batch b).
         // Up to 8 GB per buffer where HBM is plentiful: fewer, longer search launches (3 M rather than 750 k pairs per launch was faster in an A/B run)
-        uint64_t per_buf = c->prep_bytes / 4;
+        uint64_t per_buf = c->prep.cap / 4;
         if (per_buf < (8ull << 30) && per_buf < n * (uint64_t)pstride) {       // (re)allocate: what this launch needs, at least 1 GB, at most 8 GB or 1/16 of the free memory
-            size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to)); fr += c->prep_bytes;
+            size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to)); fr += c->prep.cap;
             const uint64_t lim = std::max<uint64_t>(64ull << 20, std::min<uint64_t>(8ull << 30, fr / 16));
             const uint64_t want = std::min<uint64_t>(lim, std::max<uint64_t>(1ull << 30, n * (uint64_t)pstride + (n * (uint64_t)pstride) / 4));
-            if (want > per_buf) {
-                if (c->d_prep) cudaFree(c->d_prep); c->d_prep = nullptr; c->prep_bytes = 0;
-                CK(cudaMalloc((void**)&c->d_prep, (size_t)want * 4)); c->prep_bytes = (size_t)want * 4; per_buf = want;
-            }
+            if (want > per_buf) { if ((rc = c->prep.grow((size_t)want * 4))) return rc; per_buf = want; }
         }
         sub = std::max<uint64_t>(1024, per_buf / pstride);
         if (const char* v = getenv("KJ_SPLIT_SUB")) { const long long x = atoll(v); if (x >= 1024 && (uint64_t)x < sub) sub = (uint64_t)x; }
@@ -500,28 +509,29 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     // one kernel launch over items [b0, b1), claimed through the counter `ctr` (zeroed on the launch's stream first)
     auto run = [&](KjKernel k, cudaStream_t s, unsigned long long* ctr, uint8_t* pbuf, uint64_t b0, uint64_t b1) -> int {
         CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), s));
-        k<<<grid, KJ_WARPS_PER_CTA * 32, smem, s>>>(dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, b1, d_tax, d_best, d_ids, d_nids, d_compact,
-                                                     ctr, c->d_spill[slot], c->d_gscratch[slot], kj_greedy_scratch_bytes(rp), rp.ws_global ? c->d_ws[slot] : nullptr,
-                                                     d_count_dst, c->d_err, d_acc, d_nacc, d_frag, frag_stride, d_fraglen, pbuf, pstride, b0);
+        k<<<grid, KJ_WARPS_PER_CTA * 32, smem, s>>>(dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, b1, o.tax, o.best, o.ids, o.nids, o.compact,
+                                                     ctr, S.spill.as<KjKept>(), S.gscratch.as<uint8_t>(), kj_greedy_scratch_bytes(rp), rp.ws_global ? S.ws.as<uint8_t>() : nullptr,
+                                                     o.counts, c->err.as<uint32_t>(), o.acc, o.nacc, o.frag, o.frag_stride, o.fraglen, pbuf, pstride, b0);
         c->launches++;
         return KJ_OK;
     };
+    unsigned long long* counter = c->counter.as<unsigned long long>();
     if (split) {
         // front end on the slot's own stream, search on the caller's: F(b) -> S(b) through ev_f, S(b) -> F(b+2) (same buffer) through ev_s.
         // (A search grid that leaves one CTA slot per SM to the front end of the next sub-batch was slower in an A/B run.)
-        cudaStream_t fs = c->fstream[slot]; uint8_t* base = c->d_prep + (size_t)slot * (c->prep_bytes / 2); uint64_t k = 0;
-        CK(cudaEventRecord(c->ev_in[slot], st)); CK(cudaStreamWaitEvent(fs, c->ev_in[slot], 0));      // the inputs may have been produced on the caller's stream
+        cudaStream_t fs = S.fstream; uint8_t* base = c->prep.as<uint8_t>() + (size_t)slot * (c->prep.cap / 2); uint64_t k = 0;
+        CK(cudaEventRecord(S.ev_in, st)); CK(cudaStreamWaitEvent(fs, S.ev_in, 0));      // the inputs may have been produced on the caller's stream
         for (uint64_t b0 = 0; b0 < n; b0 += sub, k++) {
             const uint64_t b1 = std::min(n, b0 + sub); const int pb = (int)(k & 1);
-            uint8_t* pbuf = base + (size_t)pb * (c->prep_bytes / 4);
-            CK(cudaStreamWaitEvent(fs, c->ev_s[slot][pb], 0));                 // the search that last read this buffer (of this or an earlier launch; no-op if none)
-            if ((rc = run(front, fs, c->d_counter + 2 + slot, pbuf, b0, b1))) return rc;
-            CK(cudaEventRecord(c->ev_f[slot][pb], fs));
-            CK(cudaStreamWaitEvent(st, c->ev_f[slot][pb], 0));
-            if ((rc = run(kern, st, c->d_counter + slot, pbuf, b0, b1))) return rc;
-            CK(cudaEventRecord(c->ev_s[slot][pb], st));
+            uint8_t* pbuf = base + (size_t)pb * (c->prep.cap / 4);
+            CK(cudaStreamWaitEvent(fs, S.ev_s[pb], 0));                 // the search that last read this buffer (of this or an earlier launch; no-op if none)
+            if ((rc = run(front, fs, counter + 2 + slot, pbuf, b0, b1))) return rc;
+            CK(cudaEventRecord(S.ev_f[pb], fs));
+            CK(cudaStreamWaitEvent(st, S.ev_f[pb], 0));
+            if ((rc = run(kern, st, counter + slot, pbuf, b0, b1))) return rc;
+            CK(cudaEventRecord(S.ev_s[pb], st));
         }
-    } else if ((rc = run(kern, st, c->d_counter + slot, nullptr, 0, n))) return rc;
+    } else if ((rc = run(kern, st, counter + slot, nullptr, 0, n))) return rc;
     CK(cudaGetLastError());
     if (time_it) CK(cudaEventRecord(c->ev_b, st));
     return KJ_OK;
@@ -535,9 +545,9 @@ static int count_taxa(kj_ctx* c, const uint64_t* d_tax, uint64_t n, unsigned lon
 }
 
 static int check_err_flag(kj_ctx* c) {
-    uint32_t e = 0; CK(cudaMemcpy(&e, c->d_err, sizeof e, cudaMemcpyDeviceToHost));
+    uint32_t e = 0; CK(cudaMemcpy(&e, c->err.p, sizeof e, cudaMemcpyDeviceToHost));
     if (e) {
-        CK(cudaMemset(c->d_err, 0, sizeof e));
+        CK(cudaMemset(c->err.p, 0, sizeof e));
         // flag 4 = the Greedy variant ring of some read was full: the next launch gets a ring 4x as large (the reference's heap is unbounded)
         if ((e & 4u) && c->variant_boost < 256u) c->variant_boost *= 4u;
         char b[160]; snprintf(b, sizeof b, "per-read work queue overflow on the device (flags 0x%x)%s", e, (e & 4u) ? "; the variant ring was enlarged, call again" : (e & 128u) ? "; the fragment strings of a read exceed frag_stride" : ""); kj_err() = b;
@@ -553,13 +563,14 @@ extern "C" int kj_classify_device2(kj_ctx* c, const char* d_seq1, const uint64_t
     CK(cudaSetDevice(c->device));
     cudaStream_t st = (cudaStream_t)cuda_stream;
     if (max_len1 == 0 || (d_seq2 && max_len2 == 0)) {
-        CK(cudaMemsetAsync(c->d_maxlen, 0, 2 * sizeof(unsigned int), st));
-        kj_maxlen_kernel<<<256, 256, 0, st>>>(d_off1, n, c->d_maxlen); c->launches++;
-        if (d_seq2) { kj_maxlen_kernel<<<256, 256, 0, st>>>(d_off2, n, c->d_maxlen + 1); c->launches++; }
-        unsigned int h[2] = {0, 0}; CK(cudaMemcpyAsync(h, c->d_maxlen, sizeof h, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st));
+        unsigned int* d_maxlen = c->maxlen.as<unsigned int>();
+        CK(cudaMemsetAsync(d_maxlen, 0, 2 * sizeof(unsigned int), st));
+        kj_maxlen_kernel<<<256, 256, 0, st>>>(d_off1, n, d_maxlen); c->launches++;
+        if (d_seq2) { kj_maxlen_kernel<<<256, 256, 0, st>>>(d_off2, n, d_maxlen + 1); c->launches++; }
+        unsigned int h[2] = {0, 0}; CK(cudaMemcpyAsync(h, d_maxlen, sizeof h, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st));
         max_len1 = h[0]; max_len2 = h[1];
     }
-    return launch(c, 0, (const uint8_t*)d_seq1, d_off1, (const uint8_t*)d_seq2, d_off2, 0, 0, n, max_len1, max_len2, d_tax, d_best, st, true, nullptr, nullptr, nullptr, d_compact);
+    return launch(c, 0, (const uint8_t*)d_seq1, d_off1, (const uint8_t*)d_seq2, d_off2, 0, 0, n, max_len1, max_len2, KjOut{d_tax, d_best, d_compact}, st, true);
 }
 
 extern "C" int kj_classify_device(kj_ctx* c, const char* d_seq1, const uint64_t* d_off1, const char* d_seq2, const uint64_t* d_off2, uint64_t n,
@@ -568,27 +579,9 @@ extern "C" int kj_classify_device(kj_ctx* c, const char* d_seq1, const uint64_t*
     return kj_classify_device2(c, d_seq1, d_off1, d_seq2, d_off2, n, max_len1, max_len2, d_tax, d_best, nullptr, cuda_stream);
 }
 
-static int ensure_staging(kj_ctx* c, int slot, size_t bytes1, size_t bytes2, size_t reads) {
-    size_t need[2] = {bytes1, bytes2};
-    for (int m = 0; m < 2; m++) if (need[m] > c->d_seq_cap[slot][m]) {
-        if (c->d_seq[slot][m]) cudaFree(c->d_seq[slot][m]); c->d_seq[slot][m] = nullptr;
-        size_t cap = need[m] + need[m] / 8 + 4096; CK(cudaMalloc((void**)&c->d_seq[slot][m], cap)); c->d_seq_cap[slot][m] = cap;
-    }
-    if (reads > c->d_reads_cap) {
-        for (int s = 0; s < 2; s++) {
-            for (int m = 0; m < 2; m++) { if (c->d_off[s][m]) cudaFree(c->d_off[s][m]); c->d_off[s][m] = nullptr; CK(cudaMalloc((void**)&c->d_off[s][m], (reads + 1) * sizeof(uint64_t))); }
-            if (c->d_tax[s]) cudaFree(c->d_tax[s]); if (c->d_best[s]) cudaFree(c->d_best[s]); c->d_tax[s] = nullptr; c->d_best[s] = nullptr;
-            CK(cudaMalloc((void**)&c->d_tax[s], reads * sizeof(uint64_t))); CK(cudaMalloc((void**)&c->d_best[s], reads * sizeof(uint32_t)));
-        }
-        c->d_reads_cap = reads;
-    }
-    return KJ_OK;
-}
-
-static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n,
-                         uint64_t* taxon_out, uint32_t* best_out, uint64_t* ids_out, uint8_t* nids_out, uint32_t* d_compact = nullptr,
-                         uint32_t* acc_out = nullptr, uint8_t* nacc_out = nullptr, char* frag_out = nullptr, uint32_t frag_stride = 0, uint32_t* frag_len_out = nullptr) {
-    if (!c || !seq1 || !off1 || !taxon_out || (seq2 && !off2) || ((ids_out == nullptr) != (nids_out == nullptr))) { kj_err() = "kj_classify: null argument"; return KJ_ERR_ARG; }
+// `o` holds the caller's host arrays (and a device array for `compact`)
+static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n, const KjOut& o) {
+    if (!c || !seq1 || !off1 || !o.tax || (seq2 && !off2) || ((o.ids == nullptr) != (o.nids == nullptr))) { kj_err() = "kj_classify: null argument"; return KJ_ERR_ARG; }
     if (n == 0) return KJ_OK;
     CK(cudaSetDevice(c->device));
     const bool paired = seq2 != nullptr;
@@ -603,36 +596,28 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
         for (auto& x : th) x.join();
         for (unsigned t = 0; t < nthr; t++) { max1 = std::max(max1, m1[t]); max2 = std::max(max2, m2[t]); }
     }
-    CK(cudaMemset(c->d_counts_pending, 0, (size_t)c->n_counts * 8));                // counts of this call: committed only if the whole call succeeds
+    CK(cudaMemset(c->counts_pending.p, 0, (size_t)c->n_counts * 8));                // counts of this call: committed only if the whole call succeeds
     uint64_t chunk_reads = KJ_CHUNK_READS;
     if (const char* v = getenv("KJ_CHUNK_READS")) { long x = atol(v); if (x >= 1024 && x <= (1 << 24)) chunk_reads = (uint64_t)x; }       // tuning hook
-    int rc = ensure_staging(c, 0, 0, 0, std::min<uint64_t>(n, chunk_reads)); if (rc) return rc;
-    if (ids_out && c->d_ids_cap < c->d_reads_cap) {
-        for (int s = 0; s < 2; s++) {
-            if (c->d_ids[s]) cudaFree(c->d_ids[s]); if (c->d_nids[s]) cudaFree(c->d_nids[s]); c->d_ids[s] = nullptr; c->d_nids[s] = nullptr;
-            CK(cudaMalloc((void**)&c->d_ids[s], c->d_reads_cap * KJ_MAX_IDS * sizeof(uint64_t))); CK(cudaMalloc((void**)&c->d_nids[s], c->d_reads_cap));
-        }
-        c->d_ids_cap = c->d_reads_cap;
+    if (o.acc || o.frag) {
+        if (o.acc && !c->sa_acc.p) { kj_err() = "kj_classify_verbose2: the context was created without kj_index_view.seq_accession"; return KJ_ERR_UNSUPPORTED; }
+        if ((o.acc && !o.nacc) || (o.frag && (!o.fraglen || o.frag_stride < 16))) { kj_err() = "kj_classify_verbose2: null argument"; return KJ_ERR_ARG; }
     }
-    if (acc_out || frag_out) {
-        if (acc_out && !c->d_sa_acc) { kj_err() = "kj_classify_verbose2: the context was created without kj_index_view.seq_accession"; return KJ_ERR_UNSUPPORTED; }
-        if ((acc_out && !nacc_out) || (frag_out && (!frag_len_out || frag_stride < 16))) { kj_err() = "kj_classify_verbose2: null argument"; return KJ_ERR_ARG; }
-        if (c->d_v2_cap < c->d_reads_cap || c->d_frag_stride < frag_stride) {
-            for (int s = 0; s < 2; s++) {
-                if (c->d_acc[s]) cudaFree(c->d_acc[s]); if (c->d_nacc[s]) cudaFree(c->d_nacc[s]); if (c->d_frag[s]) cudaFree(c->d_frag[s]); if (c->d_fraglen[s]) cudaFree(c->d_fraglen[s]);
-                c->d_acc[s] = nullptr; c->d_nacc[s] = nullptr; c->d_frag[s] = nullptr; c->d_fraglen[s] = nullptr;
-                CK(cudaMalloc((void**)&c->d_acc[s], c->d_reads_cap * KJ_MAX_MATCH_ACC * 4)); CK(cudaMalloc((void**)&c->d_nacc[s], c->d_reads_cap));
-                CK(cudaMalloc((void**)&c->d_frag[s], c->d_reads_cap * (size_t)frag_stride)); CK(cudaMalloc((void**)&c->d_fraglen[s], c->d_reads_cap * 4));
-            }
-            c->d_v2_cap = c->d_reads_cap; c->d_frag_stride = frag_stride;
-        }
+    // per-read arrays of both slots, for the largest chunk
+    const size_t reads = std::min<uint64_t>(n, chunk_reads); int rc;
+    for (KjSlot& S : c->slot) {
+        if ((rc = S.off[0].grow((reads + 1) * sizeof(uint64_t))) || (rc = S.off[1].grow((reads + 1) * sizeof(uint64_t))) ||
+            (rc = S.tax.grow(reads * sizeof(uint64_t))) || (rc = S.best.grow(reads * sizeof(uint32_t)))) return rc;
+        if (o.ids && ((rc = S.ids.grow(reads * KJ_MAX_IDS * sizeof(uint64_t))) || (rc = S.nids.grow(reads)))) return rc;
+        if (o.acc && ((rc = S.acc.grow(reads * KJ_MAX_MATCH_ACC * 4)) || (rc = S.nacc.grow(reads)))) return rc;
+        if (o.frag && ((rc = S.frag.grow(reads * (size_t)o.frag_stride)) || (rc = S.fraglen.grow(reads * 4)))) return rc;
     }
     // software pipeline over chunks: H2D + kernel + D2H of chunk k on stream k&1 overlap with chunk k+1
     const bool trace = getenv("KJ_TRACE") != nullptr;            // developer hook: per-chunk timeline on stderr
     struct Tr { cudaEvent_t e[4]; double host_ms; uint64_t cnt; }; std::vector<Tr> tr; cudaEvent_t tr0 = nullptr; const auto th0 = std::chrono::steady_clock::now();
-    if (trace) { cudaEventCreate(&tr0); cudaEventRecord(tr0, c->stream[0]); }
+    if (trace) { cudaEventCreate(&tr0); cudaEventRecord(tr0, c->slot[0].stream); }
     for (uint64_t start = 0, k = 0, cnt = 0; start < n; start += cnt, k++) {
-        const int s = (int)(k & 1); cudaStream_t st = c->stream[s];
+        KjSlot& S = c->slot[k & 1]; cudaStream_t st = S.stream;
         cnt = std::min<uint64_t>(chunk_reads, n - start);
         // long reads: bound the bases per chunk as well (at least one read)
         {
@@ -644,36 +629,41 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
         CK(cudaStreamSynchronize(st));                      // slot s free again (its previous D2H has landed)
         if (trace) { Tr t; for (auto& e : t.e) cudaEventCreate(&e); t.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - th0).count(); t.cnt = 0; tr.push_back(t); cudaEventRecord(tr.back().e[0], st); }
         const uint64_t b1 = off1[start], e1 = off1[start + cnt], b2 = paired ? off2[start] : 0, e2 = paired ? off2[start + cnt] : 0;
-        rc = ensure_staging(c, s, (size_t)(e1 - b1), (size_t)(e2 - b2), c->d_reads_cap); if (rc) return rc;
-        CK(cudaMemcpyAsync(c->d_seq[s][0], seq1 + b1, (size_t)(e1 - b1), cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(c->d_off[s][0], off1 + start, (cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+        const size_t bytes1 = (size_t)(e1 - b1), bytes2 = (size_t)(e2 - b2);      // staging bases with 1/8 slack
+        if ((rc = S.seq[0].grow(bytes1, bytes1 + bytes1 / 8 + 4096)) || (rc = S.seq[1].grow(bytes2, bytes2 + bytes2 / 8 + 4096))) return rc;
+        CK(cudaMemcpyAsync(S.seq[0].p, seq1 + b1, bytes1, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(S.off[0].p, off1 + start, (cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
         if (paired) {
-            CK(cudaMemcpyAsync(c->d_seq[s][1], seq2 + b2, (size_t)(e2 - b2), cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_off[s][1], off2 + start, (cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(S.seq[1].p, seq2 + b2, bytes2, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(S.off[1].p, off2 + start, (cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
         }
         if (trace) { tr.back().cnt = cnt; cudaEventRecord(tr.back().e[1], st); }
-        rc = launch(c, s, c->d_seq[s][0], c->d_off[s][0], paired ? c->d_seq[s][1] : nullptr, paired ? c->d_off[s][1] : nullptr, b1, b2, cnt, max1, max2,
-                    c->d_tax[s], best_out ? c->d_best[s] : nullptr, st, true, ids_out ? c->d_ids[s] : nullptr, ids_out ? c->d_nids[s] : nullptr, c->d_counts_pending, d_compact ? d_compact + start : nullptr,
-                    acc_out ? c->d_acc[s] : nullptr, acc_out ? c->d_nacc[s] : nullptr, frag_out ? c->d_frag[s] : nullptr, frag_stride, frag_out ? c->d_fraglen[s] : nullptr);
-        if (rc) return rc;
+        KjOut d;
+        d.tax = S.tax.as<uint64_t>(); d.best = o.best ? S.best.as<uint32_t>() : nullptr; d.compact = o.compact ? o.compact + start : nullptr;
+        if (o.ids) { d.ids = S.ids.as<uint64_t>(); d.nids = S.nids.as<uint8_t>(); }
+        if (o.acc) { d.acc = S.acc.as<uint32_t>(); d.nacc = S.nacc.as<uint8_t>(); }
+        if (o.frag) { d.frag = S.frag.as<char>(); d.fraglen = S.fraglen.as<uint32_t>(); }
+        d.frag_stride = o.frag_stride; d.counts = c->counts_pending.as<unsigned long long>();
+        if ((rc = launch(c, (int)(k & 1), S.seq[0].as<uint8_t>(), S.off[0].as<uint64_t>(), paired ? S.seq[1].as<uint8_t>() : nullptr, paired ? S.off[1].as<uint64_t>() : nullptr,
+                         b1, b2, cnt, max1, max2, d, st, true))) return rc;
         if (trace) cudaEventRecord(tr.back().e[2], st);
-        CK(cudaMemcpyAsync(taxon_out + start, c->d_tax[s], cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-        if (best_out) CK(cudaMemcpyAsync(best_out + start, c->d_best[s], cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-        if (ids_out) {
-            CK(cudaMemcpyAsync(ids_out + start * KJ_MAX_IDS, c->d_ids[s], cnt * KJ_MAX_IDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(nids_out + start, c->d_nids[s], cnt, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(o.tax + start, d.tax, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        if (o.best) CK(cudaMemcpyAsync(o.best + start, d.best, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        if (o.ids) {
+            CK(cudaMemcpyAsync(o.ids + start * KJ_MAX_IDS, d.ids, cnt * KJ_MAX_IDS * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(o.nids + start, d.nids, cnt, cudaMemcpyDeviceToHost, st));
         }
-        if (acc_out) {
-            CK(cudaMemcpyAsync(acc_out + start * KJ_MAX_MATCH_ACC, c->d_acc[s], cnt * KJ_MAX_MATCH_ACC * 4, cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(nacc_out + start, c->d_nacc[s], cnt, cudaMemcpyDeviceToHost, st));
+        if (o.acc) {
+            CK(cudaMemcpyAsync(o.acc + start * KJ_MAX_MATCH_ACC, d.acc, cnt * KJ_MAX_MATCH_ACC * 4, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(o.nacc + start, d.nacc, cnt, cudaMemcpyDeviceToHost, st));
         }
-        if (frag_out) {
-            CK(cudaMemcpyAsync(frag_out + start * (size_t)frag_stride, c->d_frag[s], cnt * (size_t)frag_stride, cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(frag_len_out + start, c->d_fraglen[s], cnt * 4, cudaMemcpyDeviceToHost, st));
+        if (o.frag) {
+            CK(cudaMemcpyAsync(o.frag + start * (size_t)o.frag_stride, d.frag, cnt * (size_t)o.frag_stride, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(o.fraglen + start, d.fraglen, cnt * 4, cudaMemcpyDeviceToHost, st));
         }
     }
-    if (trace && !tr.empty()) cudaEventRecord(tr.back().e[3], c->stream[(tr.size() - 1) & 1]);
-    CK(cudaStreamSynchronize(c->stream[0])); CK(cudaStreamSynchronize(c->stream[1]));
+    if (trace && !tr.empty()) cudaEventRecord(tr.back().e[3], c->slot[(tr.size() - 1) & 1].stream);
+    CK(cudaStreamSynchronize(c->slot[0].stream)); CK(cudaStreamSynchronize(c->slot[1].stream));
     if (trace) {
         fprintf(stderr, "KJ_TRACE chunk reads host_issue_ms h2d_start h2d_end kernel_end (ms since call start, device)\n");
         for (size_t k = 0; k < tr.size(); k++) { float a = 0, b = 0, d = 0; cudaEventElapsedTime(&a, tr0, tr[k].e[0]); cudaEventElapsedTime(&b, tr0, tr[k].e[1]); cudaEventElapsedTime(&d, tr0, tr[k].e[2]);
@@ -682,30 +672,28 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
     }
     rc = check_err_flag(c);
     // the per-taxon counts of this call become visible only if the whole call succeeded (a repeated call must not count twice)
-    if (rc) { CK(cudaMemset(c->d_counts_pending, 0, (size_t)c->n_counts * 8)); return rc; }
-    kj_count_commit<<<c->sm_count, 256, 0, c->stream[0]>>>(c->d_counts, c->d_counts_pending, c->n_counts); c->launches++;
-    CK(cudaStreamSynchronize(c->stream[0]));
+    if (rc) { CK(cudaMemset(c->counts_pending.p, 0, (size_t)c->n_counts * 8)); return rc; }
+    kj_count_commit<<<c->sm_count, 256, 0, c->slot[0].stream>>>(c->counts.as<unsigned long long>(), c->counts_pending.as<unsigned long long>(), c->n_counts); c->launches++;
+    CK(cudaStreamSynchronize(c->slot[0].stream));
     return KJ_OK;
 }
 
 // A full Greedy variant ring (flag 4) enlarges the ring for the next launch: repeat the call until it fits (bounded).
-static int classify_host_retry(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n,
-                               uint64_t* taxon_out, uint32_t* best_out, uint64_t* ids_out, uint8_t* nids_out, uint32_t* d_compact = nullptr,
-                               uint32_t* acc_out = nullptr, uint8_t* nacc_out = nullptr, char* frag_out = nullptr, uint32_t frag_stride = 0, uint32_t* frag_len_out = nullptr) {
+static int classify_host_retry(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n, const KjOut& o) {
     for (;;) {
         const uint32_t boost = c ? c->variant_boost : 0;
-        int rc = classify_host(c, seq1, off1, seq2, off2, n, taxon_out, best_out, ids_out, nids_out, d_compact, acc_out, nacc_out, frag_out, frag_stride, frag_len_out);
+        int rc = classify_host(c, seq1, off1, seq2, off2, n, o);
         if (rc != KJ_ERR_OVERFLOW || !c || c->variant_boost == boost) return rc;
     }
 }
 
 extern "C" int kj_classify(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n,
                            uint64_t* taxon_out, uint32_t* best_out) {
-    return classify_host_retry(c, seq1, off1, seq2, off2, n, taxon_out, best_out, nullptr, nullptr);
+    return classify_host_retry(c, seq1, off1, seq2, off2, n, KjOut{taxon_out, best_out});
 }
 extern "C" int kj_classify2(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n,
                             uint64_t* taxon_out, uint32_t* best_out, uint32_t* d_compact_out) {
-    return classify_host_retry(c, seq1, off1, seq2, off2, n, taxon_out, best_out, nullptr, nullptr, d_compact_out);
+    return classify_host_retry(c, seq1, off1, seq2, off2, n, KjOut{taxon_out, best_out, d_compact_out});
 }
 // In-process multi-GPU (the drop-in counterpart of the reference's `-z N` consumer threads, kaiju.cpp:250-257): contiguous shards of the batch,
 // one host thread per context, results written straight into the caller's arrays.  No exchange between the GPUs: reads are independent.
@@ -728,13 +716,13 @@ extern "C" int kj_device_count(void) { int n = 0; return cudaGetDeviceCount(&n) 
 extern "C" int kj_classify_verbose(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n,
                                    uint64_t* taxon_out, uint32_t* best_out, uint64_t* ids_out, uint8_t* nids_out) {
     if (!ids_out || !nids_out) { kj_err() = "kj_classify_verbose: null argument"; return KJ_ERR_ARG; }
-    return classify_host_retry(c, seq1, off1, seq2, off2, n, taxon_out, best_out, ids_out, nids_out);
+    return classify_host_retry(c, seq1, off1, seq2, off2, n, KjOut{taxon_out, best_out, nullptr, ids_out, nids_out});
 }
 
 extern "C" int kj_classify_verbose2(kj_ctx* c, const char* seq1, const uint64_t* off1, const char* seq2, const uint64_t* off2, uint64_t n, uint64_t* taxon_out, uint32_t* best_out,
                                     uint64_t* ids_out, uint8_t* nids_out, uint32_t* acc_out, uint8_t* nacc_out, char* frag_out, uint32_t frag_stride, uint32_t* frag_len_out) {
     if (!ids_out || !nids_out || !best_out) { kj_err() = "kj_classify_verbose2: null argument"; return KJ_ERR_ARG; }
-    return classify_host_retry(c, seq1, off1, seq2, off2, n, taxon_out, best_out, ids_out, nids_out, nullptr, acc_out, nacc_out, frag_out, frag_stride, frag_len_out);
+    return classify_host_retry(c, seq1, off1, seq2, off2, n, KjOut{taxon_out, best_out, nullptr, ids_out, nids_out, acc_out, nacc_out, frag_out, frag_stride, frag_len_out});
 }
 extern "C" uint64_t kj_kernel_launches(const kj_ctx* c) { return c ? c->launches : 0; }
 extern "C" uint64_t kj_index_bytes(const kj_ctx* c) { return c ? c->index_bytes : 0; }
@@ -746,18 +734,18 @@ extern "C" double kj_last_kernel_ms(const kj_ctx* c) {
 }
 extern "C" int kj_counts_reset(kj_ctx* c) {
     if (!c) return KJ_ERR_ARG; CK(cudaSetDevice(c->device));
-    CK(cudaMemset(c->d_counts, 0, (size_t)c->n_counts * 8)); return KJ_OK;
+    CK(cudaMemset(c->counts.p, 0, (size_t)c->n_counts * 8)); return KJ_OK;
 }
 extern "C" uint64_t kj_counts_size(const kj_ctx* c) { return c ? c->n_counts : 0; }
-extern "C" void* kj_counts_device_ptr(kj_ctx* c) { return c ? (void*)c->d_counts : nullptr; }
+extern "C" void* kj_counts_device_ptr(kj_ctx* c) { return c ? c->counts.p : nullptr; }
 extern "C" int kj_counts_add_device(kj_ctx* c, const uint64_t* d_taxon, uint64_t n, void* cuda_stream) {
     if (!c || (!d_taxon && n)) { kj_err() = "kj_counts_add_device: null argument"; return KJ_ERR_ARG; }
-    CK(cudaSetDevice(c->device)); return count_taxa(c, d_taxon, n, c->d_counts, (cudaStream_t)cuda_stream);
+    CK(cudaSetDevice(c->device)); return count_taxa(c, d_taxon, n, c->counts.as<unsigned long long>(), (cudaStream_t)cuda_stream);
 }
 extern "C" int kj_counts_get(kj_ctx* c, uint64_t* taxon_ids_out, uint64_t* counts_out) {
     if (!c || !counts_out) { kj_err() = "kj_counts_get: null argument"; return KJ_ERR_ARG; }
     CK(cudaSetDevice(c->device)); CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(counts_out, c->d_counts, (size_t)c->n_counts * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(counts_out, c->counts.p, (size_t)c->n_counts * 8, cudaMemcpyDeviceToHost));
     if (taxon_ids_out) { for (uint32_t i = 0; i + 1 < c->n_counts; i++) taxon_ids_out[i] = c->H.tax_id[i]; taxon_ids_out[c->n_counts - 1] = 0; }
     return KJ_OK;
 }

@@ -265,15 +265,12 @@ __global__ void kj_fmt_write(const uint64_t* __restrict__ tax, const uint32_t* _
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-struct KjDevBuf {   // grow-only device buffer
-    void* p = nullptr; size_t cap = 0; float boost = 1.f;     // boost: allocate for a batch that many times as large (cudaFree waits for every running kernel: avoid regrowth while the batches ramp up)
-    int need(size_t bytes) { if (bytes <= cap) return KJ_OK; if (p) cudaFree(p); p = nullptr; cap = 0; size_t c = (size_t)((double)bytes * boost) + bytes / 4 + 4096; CK(cudaMalloc(&p, c)); cap = c; return KJ_OK; }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <class T> T* as() const { return (T*)p; }
-};
-static int kj_scan_u32(uint32_t* d, uint64_t n, KjDevBuf& tmp, uint32_t* d_total, cudaStream_t st) {
+// Room for `bytes` in an ingest buffer, grown with slack; boost: allocate for a batch that many times as large (cudaFree waits for every
+// running kernel: avoid regrowth while the batches ramp up)
+static int kj_need(KjDevBuf& b, size_t bytes, float boost = 1.f) { return b.grow(bytes, (size_t)((double)bytes * boost) + bytes / 4 + 4096); }
+static int kj_scan_u32(uint32_t* d, uint64_t n, KjDevBuf& tmp, float boost, uint32_t* d_total, cudaStream_t st) {
     const uint32_t nb = (uint32_t)((n + KJ_SCAN_TILE - 1) / KJ_SCAN_TILE);
-    int rc = tmp.need((size_t)(nb + 1) * sizeof(uint32_t)); if (rc) return rc;
+    int rc = kj_need(tmp, (size_t)(nb + 1) * sizeof(uint32_t), boost); if (rc) return rc;
     kj_scan_reduce<<<nb, 256, 0, st>>>(d, n, tmp.as<uint32_t>());
     kj_scan_blocks<<<1, 1024, 0, st>>>(tmp.as<uint32_t>(), nb, d_total);
     kj_scan_apply<<<nb, 256, 0, st>>>(d, n, tmp.as<uint32_t>());
@@ -297,14 +294,13 @@ struct KjParsed {   // one side (file) of a chunk while it is parsed
     KjDevBuf line_start, cnt, hdr, nlen, tiles, scan_tmp, rec_pos, totals, phase, phase_tiles;
     int fastq = -1;                                              // file type, fixed by the first byte of the file
     uint64_t n_lines = 0, n_rec = 0, consumed = 0; bool eof = false, skip_all = false;
-    void release() { for (KjDevBuf* b : {&text[0], &text[1], &line_start, &cnt, &hdr, &nlen, &tiles, &scan_tmp, &rec_pos, &totals, &phase, &phase_tiles}) b->release(); }
 };
 
 // Parse the complete records in P.text[P.cur][0, P.nbytes) into O.  Sets P.n_rec; *launches counts the kernels.
-// exact: FASTQ with blank lines between records (phases from the automaton scan instead of line number mod 4).
+// exact: FASTQ with blank lines between records (phases from the automaton scan instead of line number mod 4).  boost: the batch's (kj_need).
 // Both files of a pair go through the three stages together: the parser's stream synchronises three times per batch (line count, totals, end), not
 // three times per file -- each host round trip is a gap in which the persistent classify grid of the other pipeline stage takes every free SM slot.
-static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfiles, const std::string* fn, cudaStream_t st, uint32_t* d_perr, uint64_t* launches, bool exact) {
+static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfiles, const std::string* fn, cudaStream_t st, uint32_t* d_perr, uint64_t* launches, bool exact, float boost) {
     int rc; bool on[2] = {false, false}; uint32_t ntiles[2] = {0, 0}, nl[2] = {0, 0}, h[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}; uint8_t end_phase[2] = {0, 0}; const uint8_t* phase[2] = {nullptr, nullptr};
     const int blocks = sm_count * 8;
     // stage 0: file type (first batch of a file only), newline counts
@@ -327,9 +323,9 @@ static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfile
             else { kj_err() = "Auto-detection of file type for file " + fn[f] + " failed."; return KJ_ERR_IO; }                 // kaiju.cpp:296-299
         }
         ntiles[f] = (uint32_t)((P.nbytes + KJ_NL_TILE - 1) / KJ_NL_TILE);
-        if ((rc = P.tiles.need((size_t)(ntiles[f] + 1) * 4)) || (rc = P.totals.need(64))) return rc;
+        if ((rc = kj_need(P.tiles, (size_t)(ntiles[f] + 1) * 4, boost)) || (rc = kj_need(P.totals, 64))) return rc;
         kj_nl_count<<<ntiles[f], 256, 0, st>>>(text, P.nbytes, P.tiles.as<uint32_t>());
-        if ((rc = kj_scan_u32(P.tiles.as<uint32_t>(), ntiles[f], P.scan_tmp, P.totals.as<uint32_t>() + 0, st))) return rc;
+        if ((rc = kj_scan_u32(P.tiles.as<uint32_t>(), ntiles[f], P.scan_tmp, boost, P.totals.as<uint32_t>() + 0, st))) return rc;
         CK(cudaMemcpyAsync(&nl[f], P.totals.as<uint32_t>() + 0, 4, cudaMemcpyDeviceToHost, st));
         on[f] = true; *launches += 4;
     }
@@ -342,20 +338,21 @@ static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfile
         if (nl[f] == 0) { on[f] = false; continue; }                                  // not even one complete line yet
         const char* text = P.text[P.cur].as<char>(); uint32_t* tot = P.totals.as<uint32_t>();
         const size_t L1 = (size_t)nl[f] + 1;
-        if ((rc = P.line_start.need((L1 + 1) * 8)) || (rc = P.cnt.need((L1 + 1) * 4)) || (rc = P.hdr.need((L1 + 1) * 4)) || (rc = P.nlen.need((L1 + 1) * 4))) return rc;
+        if ((rc = kj_need(P.line_start, (L1 + 1) * 8, boost)) || (rc = kj_need(P.cnt, (L1 + 1) * 4, boost)) || (rc = kj_need(P.hdr, (L1 + 1) * 4, boost)) ||
+            (rc = kj_need(P.nlen, (L1 + 1) * 4, boost))) return rc;
         kj_nl_scatter<<<ntiles[f], 256, 0, st>>>(text, P.nbytes, P.tiles.as<uint32_t>(), P.line_start.as<uint64_t>());
         KjParseDims d; d.fastq = (uint32_t)P.fastq; d.n_lines = nl[f];
         if (P.fastq && exact) {
             const uint32_t nt = (uint32_t)((L1 + KJ_FQ_TILE - 1) / KJ_FQ_TILE);
-            if ((rc = P.phase.need(L1 + 8)) || (rc = P.phase_tiles.need((size_t)(nt + 1) * 4))) return rc;
+            if ((rc = kj_need(P.phase, L1 + 8, boost)) || (rc = kj_need(P.phase_tiles, (size_t)(nt + 1) * 4, boost))) return rc;
             kj_fq_tile_maps<<<nt, 256, 0, st>>>(P.line_start.as<uint64_t>(), nl[f], P.phase_tiles.as<uint32_t>());
             kj_fq_tile_prefix<<<1, 32, 0, st>>>(P.phase_tiles.as<uint32_t>(), nt);
             kj_fq_phases<<<nt, 256, 0, st>>>(P.line_start.as<uint64_t>(), nl[f], P.phase_tiles.as<uint32_t>(), P.phase.as<uint8_t>());
             phase[f] = P.phase.as<uint8_t>(); *launches += 3;
         }
         kj_line_info<<<blocks, 256, 0, st>>>(text, P.line_start.as<uint64_t>(), d, phase[f], P.cnt.as<uint32_t>(), P.hdr.as<uint32_t>(), P.nlen.as<uint32_t>(), d_perr);
-        if ((rc = kj_scan_u32(P.cnt.as<uint32_t>(), L1, P.scan_tmp, tot + 1, st)) || (rc = kj_scan_u32(P.hdr.as<uint32_t>(), L1, P.scan_tmp, tot + 2, st)) ||
-            (rc = kj_scan_u32(P.nlen.as<uint32_t>(), L1, P.scan_tmp, tot + 3, st))) return rc;
+        if ((rc = kj_scan_u32(P.cnt.as<uint32_t>(), L1, P.scan_tmp, boost, tot + 1, st)) || (rc = kj_scan_u32(P.hdr.as<uint32_t>(), L1, P.scan_tmp, boost, tot + 2, st)) ||
+            (rc = kj_scan_u32(P.nlen.as<uint32_t>(), L1, P.scan_tmp, boost, tot + 3, st))) return rc;
         CK(cudaMemcpyAsync(h[f], tot, 16, cudaMemcpyDeviceToHost, st));
         if (phase[f]) CK(cudaMemcpyAsync(&end_phase[f], phase[f] + nl[f], 1, cudaMemcpyDeviceToHost, st));
     }
@@ -366,8 +363,8 @@ static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfile
         if (!on[f]) continue;
         const char* text = P.text[P.cur].as<char>();
         const uint64_t letters = h[f][1], headers = h[f][2], name_bytes = h[f][3];
-        if ((rc = O.seq.need(letters + 64)) || (rc = O.off.need((headers + 2) * 8)) || (rc = O.names.need(name_bytes + 64)) || (rc = O.name_off.need((headers + 2) * 4)) ||
-            (rc = P.rec_pos.need((headers + 2) * 8))) return rc;
+        if ((rc = kj_need(O.seq, letters + 64, boost)) || (rc = kj_need(O.off, (headers + 2) * 8, boost)) || (rc = kj_need(O.names, name_bytes + 64, boost)) ||
+            (rc = kj_need(O.name_off, (headers + 2) * 4, boost)) || (rc = kj_need(P.rec_pos, (headers + 2) * 8, boost))) return rc;
         KjParseDims d; d.fastq = (uint32_t)P.fastq; d.n_lines = nl[f];
         kj_line_emit<<<blocks, 256, 0, st>>>(text, P.line_start.as<uint64_t>(), d, phase[f], P.cnt.as<uint32_t>(), P.hdr.as<uint32_t>(), P.nlen.as<uint32_t>(),
                                             O.seq.as<char>(), O.off.as<uint64_t>(), O.names.as<char>(), O.name_off.as<uint32_t>(), P.rec_pos.as<uint64_t>());
@@ -427,7 +424,7 @@ struct KjFileReader {
             wgot.assign((chunk + SLICE - 1) / SLICE, 0);
             for (unsigned t = 0; t < nt; t++) workers.emplace_back([this] { worker(); });
         }
-        if ((int)ring.size() != depth) { for (auto& b : ring) b.release(); ring.assign((size_t)depth, KjDevBuf()); }
+        if ((int)ring.size() != depth) { ring.clear(); ring.resize((size_t)depth); }
         free_slots.clear(); ready.clear(); for (int k = 0; k < depth; k++) free_slots.push_back(k);
         th = std::thread([this] { run(); });
         return KJ_OK;
@@ -474,7 +471,7 @@ struct KjFileReader {
                 std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || !free_slots.empty(); }); if (stop) return;
                 ck.slot = free_slots.front(); free_slots.pop_front();
             }
-            if (ring[ck.slot].cap < chunk + 16 && ring[ck.slot].need(chunk + 16) != KJ_OK) { fail("cudaMalloc failed (staging ring)"); return; }
+            if (kj_need(ring[ck.slot], chunk + 16) != KJ_OK) { fail("cudaMalloc failed (staging ring)"); return; }
             if (got && cudaMemcpyAsync(ring[ck.slot].p, b, got, cudaMemcpyHostToDevice, stream) != cudaSuccess) { fail("cudaMemcpyAsync failed"); return; }
             cudaEventRecord(ring_ev[ck.slot], stream); cudaEventRecord(pin_ev[pb], stream); pin_busy[pb] = true; ck.ev = ring_ev[ck.slot];
             const bool last = ck.eof;
@@ -497,7 +494,7 @@ struct KjFileReader {
         for (int k = 0; k < 2; k++) { if (pin[k]) pinned->put(pin[k], chunk); pin[k] = nullptr; pin_busy[k] = false; if (pin_ev[k]) cudaEventDestroy(pin_ev[k]); pin_ev[k] = nullptr; }
         ready.clear(); free_slots.clear(); wgen = 0; wslices = 0; wnext = 0; wleft = 0;
     }
-    void release() { for (auto& b : ring) b.release(); ring.clear(); for (auto e : ring_ev) cudaEventDestroy(e); ring_ev.clear(); if (stream) cudaStreamDestroy(stream); stream = nullptr; }
+    void release() { for (auto e : ring_ev) cudaEventDestroy(e); ring_ev.clear(); if (stream) cudaStreamDestroy(stream); stream = nullptr; }
 };
 struct KjWriter {   // ordered output: pinned buffers filled by D2H copies, written by one thread
     FILE* out = nullptr; bool own = false; std::vector<char*> pool; size_t cap = 0; int nbuf = 3; std::deque<std::pair<char*, size_t>> ready; std::deque<char*> free_;
@@ -555,11 +552,8 @@ struct KjFilesState {
         if (wr_open) wr.close(); wr_open = false;
         filled.clear(); n_free = KJ_FILE_SLOTS; abort = false; lane[0].busy = lane[1].busy = false;
     }
-    void release() {       // with the context
-        for (int f = 0; f < 2; f++) { side[f].release(); rd[f].release(); }
-        for (KjBatch& b : slot) for (KjBatchSide& o : b.s) for (KjDevBuf* d : {&o.seq, &o.off, &o.names, &o.name_off}) d->release();
-        for (KjLane& l : lane) for (KjDevBuf* d : {&l.tax, &l.best, &l.ids, &l.nids, &l.len, &l.out, &l.scan_tmp, &l.totals}) d->release();
-        pstat.release(); pending2.release();
+    void release() {       // with the context; the device buffers go with their owners
+        for (int f = 0; f < 2; f++) rd[f].release();
         if (sp) cudaStreamDestroy(sp); sp = nullptr;
         pinned.release();
     }
@@ -583,13 +577,7 @@ static int kj_parse_chunks(int device, int sm_count, KjFilesState& S, size_t chu
         { std::unique_lock<std::mutex> lk(S.mu); S.cv.wait(lk, [&] { return S.abort || S.n_free > 0; }); if (S.abort) return KJ_OK; S.n_free--; }
         si = (int)(S.nbatches % KJ_FILE_SLOTS); KjBatch& B = S.slot[si]; S.nbatches++;
         S.tm[0] += kj_ms_since(t);
-        {   // buffers of the first, small batches are allocated for the final batch size
-            const float boost = target < batch_max ? (float)batch_max / (float)target : 1.f; B.boost = boost;
-            for (int f = 0; f < S.nfiles; f++) {
-                KjParsed& P = S.side[f]; for (KjDevBuf* b : {&P.line_start, &P.cnt, &P.hdr, &P.nlen, &P.tiles, &P.scan_tmp, &P.rec_pos, &P.phase, &P.phase_tiles}) b->boost = boost;
-                for (KjDevBuf* b : {&B.s[f].seq, &B.s[f].off, &B.s[f].names, &B.s[f].name_off}) b->boost = boost;
-            }
-        }
+        B.boost = target < batch_max ? (float)batch_max / (float)target : 1.f;      // buffers of the first, small batches are allocated for the final batch size
         // 1. top up both sides to `target` bytes: the carry is already at the front of the device text, staged chunks are appended behind it
         for (int f = 0; f < S.nfiles; f++) {
             KjParsed& P = S.side[f];
@@ -597,9 +585,9 @@ static int kj_parse_chunks(int device, int sm_count, KjFilesState& S, size_t chu
                 KjStaged ck = S.rd[f].next();
                 if (!ck.error.empty()) { kj_err() = ck.error; return KJ_ERR_IO; }
                 if ((P.nbytes + ck.n + 1) > P.text[P.cur].cap) {           // grow: move what is there into the larger buffer
-                    KjDevBuf nb; if ((rc = nb.need(P.nbytes + ck.n + std::max(target, batch_max) + chunk + 1))) return rc;
+                    KjDevBuf nb; if ((rc = kj_need(nb, P.nbytes + ck.n + std::max(target, batch_max) + chunk + 1))) return rc;
                     if (P.nbytes) CK(cudaMemcpyAsync(nb.p, P.text[P.cur].p, P.nbytes, cudaMemcpyDeviceToDevice, st));
-                    CK(cudaStreamSynchronize(st)); P.text[P.cur].release(); P.text[P.cur] = nb;
+                    CK(cudaStreamSynchronize(st)); P.text[P.cur] = std::move(nb);
                 }
                 CK(cudaStreamWaitEvent(st, ck.ev, 0));
                 if (ck.n) CK(cudaMemcpyAsync(P.text[P.cur].as<char>() + P.nbytes, S.rd[f].ring[ck.slot].p, ck.n, cudaMemcpyDeviceToDevice, st));
@@ -619,7 +607,7 @@ static int kj_parse_chunks(int device, int sm_count, KjFilesState& S, size_t chu
         uint64_t n = 0; bool all_eof = false; uint64_t pos[2] = {0, 0}; uint32_t hstat[4] = {0, 0, 0, 0};
         for (int pass = 0; pass < 2; pass++) {
             CK(cudaMemsetAsync(d_stat, 0, 16, st));
-            if ((rc = kj_parse_sides(sm_count, S.side, B.s, S.nfiles, fn, st, d_stat + 2, &S.parse_launches, pass == 1))) return rc;
+            if ((rc = kj_parse_sides(sm_count, S.side, B.s, S.nfiles, fn, st, d_stat + 2, &S.parse_launches, pass == 1, B.boost))) return rc;
             // (kj_parse_sides synchronises the stream: the staging buffers appended above are free again)
             for (int f = 0; f < S.nfiles; f++) { for (int sl : used[f]) S.rd[f].release_slot(sl); used[f].clear(); }
             n = S.side[0].n_rec; if (paired) n = std::min(n, S.side[1].n_rec);
@@ -646,7 +634,7 @@ static int kj_parse_chunks(int device, int sm_count, KjFilesState& S, size_t chu
         for (int f = 0; f < S.nfiles; f++) {
             KjParsed& P = S.side[f]; const uint64_t consumed = P.skip_all ? P.nbytes : (P.n_lines ? pos[f] : 0);
             const uint64_t tail = P.nbytes - consumed; const int other = P.cur ^ 1;
-            if ((rc = P.text[other].need(tail + std::max(target, batch_max) + chunk + 1))) return rc;
+            if ((rc = kj_need(P.text[other], tail + std::max(target, batch_max) + chunk + 1))) return rc;
             if (tail) CK(cudaMemcpyAsync(P.text[other].p, P.text[P.cur].as<char>() + consumed, tail, cudaMemcpyDeviceToDevice, st));
             P.cur = other; P.nbytes = tail;
         }
@@ -684,11 +672,12 @@ static int kj_classify_files_impl(kj_ctx* c, KjFilesState& S, const char* in1, c
     for (int f = 0; f < S.nfiles; f++) { if ((rc = S.rd[f].open(fn[f], chunk, depth, c->device, &S.pinned))) return rc; S.rd_open[f] = true; }
     const size_t out_cap = 16u << 20;
     if ((rc = S.wr.open(out_path, out_cap, 3, &S.pinned))) return rc; S.wr_open = true;
-    if ((rc = S.pstat.need(64)) || (rc = S.pending2.need((size_t)c->n_counts * 8 + 64))) return rc;
-    unsigned long long* pend[2] = {c->d_counts_pending, S.pending2.as<unsigned long long>()};
+    if ((rc = kj_need(S.pstat, 64)) || (rc = kj_need(S.pending2, (size_t)c->n_counts * 8 + 64))) return rc;
+    unsigned long long* pend[2] = {c->counts_pending.as<unsigned long long>(), S.pending2.as<unsigned long long>()};
     for (int l = 0; l < 2; l++) {
-        if ((rc = S.lane[l].totals.need(64))) return rc;
-        CK(cudaMemsetAsync(S.lane[l].totals.p, 0, 64, c->stream[l])); CK(cudaMemsetAsync(pend[l], 0, (size_t)c->n_counts * 8, c->stream[l])); CK(cudaStreamSynchronize(c->stream[l]));
+        if ((rc = kj_need(S.lane[l].totals, 64))) return rc;
+        cudaStream_t st = c->slot[l].stream;
+        CK(cudaMemsetAsync(S.lane[l].totals.p, 0, 64, st)); CK(cudaMemsetAsync(pend[l], 0, (size_t)c->n_counts * 8, st)); CK(cudaStreamSynchronize(st));
         S.lane[l].busy = false; S.lane[l].batch = -1;
     }
     uint64_t n_reads = 0;
@@ -706,22 +695,23 @@ static int kj_classify_files_impl(kj_ctx* c, KjFilesState& S, const char* in1, c
         KjLane& Ln = S.lane[l]; KjBatch& B = S.slot[si]; const uint64_t n = B.n; int r;
         Ln.batch = si; Ln.busy = true;
         if (!n) return KJ_OK;
-        for (KjDevBuf* b : {&Ln.tax, &Ln.best, &Ln.ids, &Ln.nids, &Ln.len, &Ln.out, &Ln.scan_tmp}) b->boost = B.boost;
-        if ((r = Ln.tax.need(n * 8)) || (r = Ln.best.need(n * 4)) || (r = Ln.len.need((n + 2) * 4))) return r;
-        if (verbose && ((r = Ln.ids.need(n * KJ_MAX_IDS * 8)) || (r = Ln.nids.need(n)))) return r;
+        if ((r = kj_need(Ln.tax, n * 8, B.boost)) || (r = kj_need(Ln.best, n * 4, B.boost)) || (r = kj_need(Ln.len, (n + 2) * 4, B.boost))) return r;
+        if (verbose && ((r = kj_need(Ln.ids, n * KJ_MAX_IDS * 8, B.boost)) || (r = kj_need(Ln.nids, n, B.boost)))) return r;
+        KjOut o; o.tax = Ln.tax.as<uint64_t>(); o.best = Ln.best.as<uint32_t>(); o.counts = pend[l];
+        if (verbose) { o.ids = Ln.ids.as<uint64_t>(); o.nids = Ln.nids.as<uint8_t>(); }
         return launch(c, l, B.s[0].seq.as<uint8_t>(), B.s[0].off.as<uint64_t>(), paired ? B.s[1].seq.as<uint8_t>() : nullptr, paired ? B.s[1].off.as<uint64_t>() : nullptr, 0, 0, n, B.maxlen[0], B.maxlen[1],
-                      Ln.tax.as<uint64_t>(), Ln.best.as<uint32_t>(), c->stream[l], false, verbose ? Ln.ids.as<uint64_t>() : nullptr, verbose ? Ln.nids.as<uint8_t>() : nullptr, pend[l]);
+                      o, c->slot[l].stream, false);
     };
     auto finish = [&](int l) -> int {                 // wait for lane l's kernel, check, count, format, write; the batch slot goes back to the parser
-        KjLane& Ln = S.lane[l]; KjBatch& B = S.slot[Ln.batch]; const uint64_t n = B.n; cudaStream_t st = c->stream[l]; int r;
+        KjLane& Ln = S.lane[l]; KjBatch& B = S.slot[Ln.batch]; const uint64_t n = B.n; cudaStream_t st = c->slot[l].stream; int r;
         if (n) {
             CK(cudaStreamSynchronize(st));
-            uint32_t e = 0; CK(cudaMemcpy(&e, c->d_err, sizeof e, cudaMemcpyDeviceToHost));
+            uint32_t e = 0; CK(cudaMemcpy(&e, c->err.p, sizeof e, cudaMemcpyDeviceToHost));
             if (e) {
                 // the error word is shared by the two lanes: let the other kernel finish, then repeat what was in flight, one launch at a time
                 // (only a full Greedy variant ring is repaired by a repeat: the ring grows)
                 const int o = l ^ 1; const bool other = S.lane[o].busy && S.slot[S.lane[o].batch].n > 0;
-                if (other) CK(cudaStreamSynchronize(c->stream[o]));
+                if (other) CK(cudaStreamSynchronize(c->slot[o].stream));
                 const uint32_t boost = c->variant_boost;
                 r = check_err_flag(c);
                 for (int k = 0; k < 2; k++) CK(cudaMemset(pend[k], 0, (size_t)c->n_counts * 8));      // failed launches do not count
@@ -730,7 +720,7 @@ static int kj_classify_files_impl(kj_ctx* c, KjFilesState& S, const char* in1, c
                     const int ll = k == 0 ? l : o; if (k == 1 && !other) break;
                     for (;;) {
                         if ((r = start(ll, S.lane[ll].batch))) return r;
-                        CK(cudaStreamSynchronize(c->stream[ll]));
+                        CK(cudaStreamSynchronize(c->slot[ll].stream));
                         const uint32_t b2 = c->variant_boost; r = check_err_flag(c);
                         if (r) CK(cudaMemset(pend[ll], 0, (size_t)c->n_counts * 8));
                         if (r == KJ_ERR_OVERFLOW && c->variant_boost != b2) continue;
@@ -741,11 +731,11 @@ static int kj_classify_files_impl(kj_ctx* c, KjFilesState& S, const char* in1, c
             }
             S.tm[6] += kj_ms_since(t);
             unsigned long long* d_nclass = (unsigned long long*)((char*)Ln.totals.p + 16);
-            kj_count_commit<<<c->sm_count, 256, 0, st>>>(c->d_counts, pend[l], c->n_counts); c->launches++;     // this batch succeeded: its reads join the per-taxon counts
+            kj_count_commit<<<c->sm_count, 256, 0, st>>>(c->counts.as<unsigned long long>(), pend[l], c->n_counts); c->launches++;     // this batch succeeded: its reads join the per-taxon counts
             kj_fmt_len<<<c->sm_count * 4, 256, 0, st>>>(Ln.tax.as<uint64_t>(), Ln.best.as<uint32_t>(), Ln.ids.as<uint64_t>(), Ln.nids.as<uint8_t>(), B.s[0].name_off.as<uint32_t>(), n, verbose, Ln.len.as<uint32_t>(), d_nclass);
-            if ((r = kj_scan_u32(Ln.len.as<uint32_t>(), n + 1, Ln.scan_tmp, (uint32_t*)Ln.totals.p, st))) return r;
+            if ((r = kj_scan_u32(Ln.len.as<uint32_t>(), n + 1, Ln.scan_tmp, B.boost, (uint32_t*)Ln.totals.p, st))) return r;
             uint32_t out_bytes = 0; CK(cudaMemcpyAsync(&out_bytes, Ln.totals.p, 4, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st));
-            if ((r = Ln.out.need(out_bytes + 64))) return r;
+            if ((r = kj_need(Ln.out, out_bytes + 64, B.boost))) return r;
             kj_fmt_write<<<c->sm_count * 4, 256, 0, st>>>(Ln.tax.as<uint64_t>(), Ln.best.as<uint32_t>(), Ln.ids.as<uint64_t>(), Ln.nids.as<uint8_t>(), B.s[0].names.as<char>(), B.s[0].name_off.as<uint32_t>(), n, verbose,
                                                        Ln.len.as<uint32_t>(), Ln.out.as<char>());
             CK(cudaGetLastError()); c->launches += 6;
@@ -793,12 +783,12 @@ extern "C" int kj_classify_files(kj_ctx* c, const char* in1, const char* in2, co
     if (!c || !in1 || !*in1) { kj_err() = "kj_classify_files: null argument"; return KJ_ERR_ARG; }
     if (c->params.input_is_protein && in2 && *in2) { kj_err() = "Protein input only supports one input file."; return KJ_ERR_ARG; }
     CK(cudaSetDevice(c->device));
-    if (!c->files) c->files = new KjFilesState();
-    KjFilesState* S = c->files;
+    if (!c->files) c->files.reset(new KjFilesState());
+    KjFilesState* S = c->files.get();
     int rc = kj_classify_files_impl(c, *S, in1, in2, out_path, verbose, n_reads, n_classified);
     const std::string keep = kj_err();
-    cudaStreamSynchronize(c->stream[0]); cudaStreamSynchronize(c->stream[1]);
+    cudaStreamSynchronize(c->slot[0].stream); cudaStreamSynchronize(c->slot[1].stream);
     S->end_call();
-    if (rc) { cudaMemset(c->d_err, 0, 4); kj_err() = keep; } else if (S->wr.failed) { kj_err() = "write error on the output file"; rc = KJ_ERR_IO; }
+    if (rc) { cudaMemset(c->err.p, 0, 4); kj_err() = keep; } else if (S->wr.failed) { kj_err() = "write error on the output file"; rc = KJ_ERR_IO; }
     return rc;
 }
