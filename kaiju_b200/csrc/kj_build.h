@@ -139,6 +139,11 @@ __global__ void kj_bld_sa_tax_scaled(const KjDevIndex* __restrict__ base_ix, uin
         sa_tax[e] = k < n_rows ? kj_sa_taxon<IdxT>(*base_ix, k / rep) : KJ_TAX_BAD;
     }
 }
+// dense row -> taxon array: every row resolved by the classify kernels' own walk (kj_row_taxon), so the array equals the walk by construction,
+// the guard entry of the sampled suffix array and the walks that end on a terminator included.  Narrow indexes only.
+__global__ void kj_bld_row_tax(const KjDevIndex* __restrict__ ix, uint64_t n_rows, uint32_t* __restrict__ row_tax) {
+    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n_rows; k += (uint64_t)gridDim.x * blockDim.x) row_tax[k] = kj_row_taxon<uint32_t>(*ix, k);
+}
 __global__ void kj_bld_repeat_u32(const uint32_t* __restrict__ src, uint64_t n_out, uint32_t rep, uint32_t* __restrict__ dst) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = src[i / rep];
 }
@@ -293,5 +298,22 @@ static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, 
     }
     CK(cudaDeviceSynchronize());
     k_out = k;
+    return KJ_OK;
+}
+
+// The dense row -> taxon array of a finished narrow index (descriptor uploaded, k-mer tables decided), when it fits next to the index with
+// KJ_ROW_TAX_MARGIN to spare.  Not for wide indexes (4 B per row next to 3.5 B of rank records) nor for the base context that kj_create_scaled
+// throws away after the construction.
+#define KJ_ROW_TAX_MARGIN (8ull << 30)
+static int kj_device_build_row_tax(kj_ctx* c, uint64_t& tot) {
+    const KjHostIndex& H = c->H;
+    if (H.wide || kj_transient_ctx) return KJ_OK;
+    const size_t bytes = (size_t)H.bwtlen * 4;
+    size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));
+    if (bytes + KJ_ROW_TAX_MARGIN > fr) return KJ_OK;
+    int rc = c->row_tax.grow(bytes); if (rc) return rc;
+    kj_bld_row_tax<<<c->sm_count * 16, 256>>>(c->ix.as<KjDevIndex>(), H.bwtlen, c->row_tax.as<uint32_t>());
+    CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches++;
+    tot += bytes;
     return KJ_OK;
 }

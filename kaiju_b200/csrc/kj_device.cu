@@ -226,6 +226,7 @@ struct kj_ctx {
     KjDevBuf ix, tables;
     KjDevBuf ix_mem, kmer_mem; int kmer_k_mem = 0;      // the MEM kernels' own descriptor: same index, 7-mer table (kj_create)
     KjDevBuf rank, letters, sa_tax, seq_tax, sa_acc, seq_acc, tax_parent, tax_depth, tax_id, lnfact, kmer;
+    KjDevBuf row_tax;              // taxon per BWT row (kj_device_build_row_tax; empty: the kernels walk)
     uint64_t index_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;
     // run state
     KjDevBuf counter, err, maxlen, quirk;
@@ -322,7 +323,7 @@ static int upload_descriptor(kj_ctx* c) {
     for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
     D.sa_acc = c->sa_acc.as<const uint32_t>(); D.seq_acc = c->seq_acc.as<const uint32_t>();
     D.sa_tax = c->sa_tax.as<const uint32_t>(); D.seq_tax = c->seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
-    D.n_sa = c->n_sa; D.nseq = H.nseq;
+    D.n_sa = c->n_sa; D.row_tax = c->row_tax.as<const uint32_t>(); D.nseq = H.nseq;
     D.tax_parent = c->tax_parent.as<const uint32_t>(); D.tax_depth = c->tax_depth.as<const uint32_t>(); D.tax_id = c->tax_id.as<const uint64_t>(); D.n_tax = (uint32_t)H.tax_id.size();
     D.lnfact = c->lnfact.as<const double>(); D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? c->kmer.p : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = c->tables.as<KjTables>();
     D.quirk_lo = H.quirk_lo; D.mono = H.quirk_lo == ~0ull ? 1 : 0; D.quirk_d = c->quirk.as<uint64_t>();
@@ -342,10 +343,12 @@ static int upload_small(kj_ctx* c, uint64_t& tot) {
     CK(cudaMemcpy(c->tables.p, &H.tables, sizeof(KjTables), cudaMemcpyHostToDevice));
     return KJ_OK;
 }
+static int kj_device_build_row_tax(kj_ctx* c, uint64_t& tot);      // kj_build.h
 static int finish_ctx(kj_ctx* c, uint64_t tot) {
     KjHostIndex& H = c->H; int rc;
     CK(cudaMemcpy(c->quirk.p, H.quirk_d, sizeof H.quirk_d, cudaMemcpyHostToDevice));
-    if ((rc = upload_descriptor(c))) return rc;
+    // the row -> taxon array is built by walking the finished index; both descriptors then carry it
+    if ((rc = upload_descriptor(c)) || (rc = kj_device_build_row_tax(c, tot)) || (rc = upload_descriptor(c))) return rc;
     c->index_bytes = tot;
     if ((rc = c->counter.grow(4 * sizeof(unsigned long long))) || (rc = c->maxlen.grow(2 * sizeof(unsigned int)))) return rc;       // counters: [slot] classify / search, [2 + slot] front end
     for (KjSlot& S : c->slot) {

@@ -14,6 +14,8 @@
 //   sa_tax     : the sampled suffix array reduced to what classification needs -- the (compact) taxon of
 //                the sequence each sampled suffix belongs to (bwt/suffixArray.h:47-51 + ConsumerThread.cpp:812-832).
 //   seq_tax    : compact taxon per sequence number (used when the LF walk runs into a terminator, bwt.c:119).
+//   row_tax    : compact taxon per BWT row (4 B per row), built on the device from the three arrays above by walking every row once:
+//                resolves a matched row with one load instead of an LF walk of ~2^sa_exp dependent steps.
 //   tax_*      : taxonomy re-indexed densely: ids present in nodes.dmp get indices [0,n_present), DB taxa
 //                absent from nodes.dmp get the indices after that (depth 0 marks "absent", util.cpp:206).
 #pragma once
@@ -57,17 +59,19 @@ struct KjTables {
     uint8_t aa_index[32];            // protein input: upper-case letter - 'A' -> alphabet index, 0 = splits the read (ConsumerThread.cpp:664)
 };
 
+// (the 32-bit members are paired so that the descriptor has no padding holes: the kernels stage it in shared memory next to the work spaces)
 struct KjDevIndex {
     const uint64_t* rank; uint64_t nb;          // [alen][nb] records of 2 (narrow) or 4 (wide) 64-bit words
     const uint64_t* rank_base[KJ_MAX_ALEN];     // records of letter c (saves the multiply in the inner loop)
     const uint64_t* letters;
-    uint64_t bwtlen; int alen;
+    uint64_t bwtlen; int alen; uint32_t nseq;
     uint64_t C[KJ_MAX_ALEN + 1];                // C[c] = first SA row of letter c; C[alen] = bwtlen
     const uint32_t* sa_tax; const uint32_t* seq_tax;
     const uint32_t* sa_acc; const uint32_t* seq_acc;     // accession rank per sampled suffix / sequence (NULL unless the index view carried seq_accession)
-    uint64_t sa_check; int sa_exp; int64_t sa_bias; uint64_t n_sa; uint32_t nseq;
-    const uint32_t* tax_parent; const uint32_t* tax_depth; const uint64_t* tax_id; uint32_t n_tax;
-    const double* lnfact; int n_lnfact;
+    uint64_t sa_check; int sa_exp; int64_t sa_bias; uint64_t n_sa;
+    const uint32_t* row_tax;                    // taxon of every BWT row, = the SA walk's result (narrow indexes that have room for it; NULL = walk)
+    const uint32_t* tax_parent; const uint32_t* tax_depth; const uint64_t* tax_id; uint32_t n_tax; int n_lnfact;
+    const double* lnfact;
     const void* kmer; int kmer_k;               // direct-address table of k-mer intervals (KjKmer32 if !wide else KjKmer; 0 = off)
     int wide;                                   // 1 if bwtlen >= 2^32 (64-bit interval arithmetic in the kernels)
     int mono;                                   // 1: true FM index (match starts monotone in the end position); 0: the reference's checkpoint quirk applies (no chain bounds)

@@ -1,0 +1,27 @@
+"""The CPU warp emulator with the dense row -> taxon array (tests/emu/kj_emu_row_tax.cpp), compiled on first use into a directory of the
+caller's choosing (test infrastructure: the library itself builds the array on the device)."""
+import ctypes as C
+import os
+import subprocess
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+
+
+def load(out_dir, params_type):
+    """ctypes handle of the emulator, built into out_dir; params_type = the kj_params ctypes structure."""
+    so = os.path.join(out_dir, "libkjemu_row_tax.so")
+    if not os.path.exists(so):
+        os.makedirs(out_dir, exist_ok=True)
+        tmp = so + ".%d" % os.getpid()
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-DKJ_EMU", "-o", tmp, os.path.join(HERE, "emu", "kj_emu_row_tax.cpp"),
+                               os.path.join(ROOT, "kaiju_b200", "csrc", "kj_host.cpp"), "-lpthread"])
+        os.replace(tmp, so)
+    E = C.CDLL(so)
+    E.kjemu_create.restype = C.c_void_p; E.kjemu_create.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(params_type)]
+    E.kjemu_destroy_row_tax.argtypes = [C.c_void_p]
+    E.kjemu_use_row_tax.argtypes = [C.c_void_p, C.c_int]
+    E.kjemu_classify.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_uint64, C.c_void_p, C.c_void_p, C.c_int]
+    E.kjemu_classify_ids.argtypes = [C.c_void_p] + [C.c_void_p] * 4 + [C.c_uint64] + [C.c_void_p] * 4 + [C.c_int]
+    E.kjemu_stats.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    return E
