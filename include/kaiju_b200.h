@@ -213,10 +213,16 @@ int kj_check_errors(kj_ctx *ctx);
 const char *kj_last_error(void);                  /* thread-local text of the last failure          */
 uint64_t kj_kernel_launches(const kj_ctx *ctx);   /* number of kernels this context has launched    */
 uint64_t kj_index_bytes(const kj_ctx *ctx);       /* bytes of HBM held by the index                 */
+/* Rank layout of the context's index: 0 narrow (< 2^32 rows, 5.25 B per row), 1 wide (64-bit intervals, 3.5 B per row plus 0.67 B of packed
+ * letters), 2 compact (64-bit intervals, 1.003 B per row, letters included).  A 64-bit index is built wide when the wide construction fits in
+ * the HBM free at creation, else compact; when neither fits, kj_create / kj_create_scaled fail with KJ_ERR_NOMEM and kj_last_error() names the
+ * bytes needed and the bytes free.  -1 for a null context. */
+int kj_index_layout(const kj_ctx *ctx);
 double kj_last_kernel_ms(const kj_ctx *ctx);      /* device time of the last classify kernel (CUDA events) */
 int kj_launch_geometry(const kj_ctx *ctx, int *grid, int *block, int *dyn_smem_bytes);  /* of the last classify launch */
 int kj_version(void);
-/* test hooks: checksums of the index arrays (rank, letters, sa_tax, seq_tax, kmer | bwtlen, wide, n_sa) as held in HBM by a context,
+/* test hooks: checksums of the index arrays (rank, letters, sa_tax, seq_tax, kmer | bwtlen, layout, n_sa) as held in HBM by a context (compact
+ * layout: the records in slot 0, the superblock table in slot 1),
  * and the same from the host transcoder (no GPU needed) -- the device construction is tested against the host one array for array */
 int kj_debug_index_checksums(kj_ctx *ctx, uint64_t out[8]);
 int kj_debug_host_index_checksums(const kj_index_view *index, const kj_taxonomy_view *taxonomy, uint64_t out[8]);

@@ -82,6 +82,8 @@ def lib():
                                          C.c_void_p, C.c_void_p, C.c_void_p]
         L.kj_kernel_launches.restype = C.c_uint64; L.kj_kernel_launches.argtypes = [C.c_void_p]
         L.kj_index_bytes.restype = C.c_uint64; L.kj_index_bytes.argtypes = [C.c_void_p]
+        if hasattr(L, "kj_index_layout"):
+            L.kj_index_layout.restype = C.c_int; L.kj_index_layout.argtypes = [C.c_void_p]
         L.kj_last_kernel_ms.restype = C.c_double; L.kj_last_kernel_ms.argtypes = [C.c_void_p]
         L.kj_classify_files.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.kj_counts_reset.argtypes = [C.c_void_p]
@@ -310,6 +312,11 @@ class Classifier:
     @property
     def index_bytes(self):
         return int(lib().kj_index_bytes(self._ctx))
+
+    @property
+    def layout(self):
+        """Rank layout of the index in HBM: 0 narrow, 1 wide, 2 compact (kj_index_layout)."""
+        return int(lib().kj_index_layout(self._ctx))
 
     @property
     def index_build_ms(self):

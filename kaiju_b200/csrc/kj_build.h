@@ -179,12 +179,133 @@ static int kj_bld_upload(void* d, const void* h, size_t bytes) {
     return KJ_OK;
 }
 
-// Builds the large arrays of the context on the device.  c->H holds the meta data (kj_build_host_meta); `base` (scaled build only) is a
-// finished context over the same index with copies = 1, whose device index resolves base suffix-array rows to taxa.
-static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcode[256], uint32_t rep, const kj_ctx* base, uint64_t& tot) {
+// ---- compact layout (kj_layout.h): one CTA per 65536-row superblock, one thread per 128-row record.  A record depends only on its own
+// superblock, so the BWT can be built a chunk of whole superblocks at a time.  `bwt` holds rows [row0, ...) (rep == 1) or the whole base BWT
+// (rep > 1: row r of the K-fold index is base row r / K).  sb_tot[s][c] = #c in superblock s (KJ_CSB_STRIDE per superblock).
+#define KJ_CSB_RECS (1u << (KJ_CSB_SHIFT - 7))
+__global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* __restrict__ bwt, const __grid_constant__ KjBuildLcode lc, uint64_t s0, uint64_t row0, uint64_t n,
+                                                                  uint32_t rep, uint64_t nb, uint64_t* __restrict__ rec_out, uint32_t* __restrict__ sb_tot) {
+    __shared__ uint8_t lcs[256];
+    __shared__ __align__(16) uint16_t cnt[KJ_CSB_RECS][KJ_MAX_ALEN];    // #c in the first half of each record, then the midpoint counts
+    __shared__ uint8_t full[KJ_CSB_RECS][KJ_MAX_ALEN];                  // #c in each record
+    lcs[threadIdx.x] = lc.v[threadIdx.x];
+    for (uint32_t i = threadIdx.x; i < KJ_CSB_RECS * KJ_MAX_ALEN; i += KJ_BLD_THREADS) { (&cnt[0][0])[i] = 0; (&full[0][0])[i] = 0; }
+    __syncthreads();
+    const uint64_t s = s0 + blockIdx.x;
+    for (uint32_t r = threadIdx.x; r < KJ_CSB_RECS; r += KJ_BLD_THREADS) {
+        const uint64_t b = (s << (KJ_CSB_SHIFT - 7)) + r;
+        if (b >= nb) break;
+        uint64_t pw[10];
+        #pragma unroll
+        for (int h = 0; h < 2; h++) {
+            uint64_t p0 = 0, p1 = 0, p2 = 0, p3 = 0, p4 = 0;
+            for (uint32_t i = 0; i < 64; i++) {
+                const uint64_t row = b * 128u + (uint32_t)h * 64u + i;
+                uint32_t l = 31;                                             // rows past the end: a letter no rank query counts
+                if (row < n) { l = lcs[bwt[rep == 1 ? row - row0 : row / rep]]; full[r][l]++; if (h == 0) cnt[r][l]++; }
+                p0 |= (uint64_t)(l & 1u) << i; p1 |= (uint64_t)((l >> 1) & 1u) << i; p2 |= (uint64_t)((l >> 2) & 1u) << i;
+                p3 |= (uint64_t)((l >> 3) & 1u) << i; p4 |= (uint64_t)((l >> 4) & 1u) << i;
+            }
+            pw[5 * h] = p0; pw[5 * h + 1] = p1; pw[5 * h + 2] = p2; pw[5 * h + 3] = p3; pw[5 * h + 4] = p4;
+        }
+        ulonglong2* o = (ulonglong2*)(rec_out + b * KJ_RANK_WORDS_COMPACT);
+        #pragma unroll
+        for (int q = 0; q < 5; q++) o[q] = make_ulonglong2(pw[2 * q], pw[2 * q + 1]);
+    }
+    __syncthreads();
+    if (threadIdx.x < KJ_MAX_ALEN) {                                     // per letter: running count over the superblock's records
+        const uint32_t c = threadIdx.x; uint32_t run = 0;
+        for (uint32_t r = 0; r < KJ_CSB_RECS; r++) { const uint32_t h = cnt[r][c]; cnt[r][c] = (uint16_t)(run + h); run += full[r][c]; }
+        sb_tot[s * KJ_CSB_STRIDE + c] = run;
+    }
+    __syncthreads();
+    for (uint32_t r = threadIdx.x; r < KJ_CSB_RECS; r += KJ_BLD_THREADS) {
+        const uint64_t b = (s << (KJ_CSB_SHIFT - 7)) + r;
+        if (b >= nb) break;
+        const ulonglong2* src = (const ulonglong2*)&cnt[r][0]; ulonglong2* o = (ulonglong2*)(rec_out + b * KJ_RANK_WORDS_COMPACT + KJ_CPT_COUNT_WORD);
+        #pragma unroll
+        for (int q = 0; q < 3; q++) o[q] = src[q];
+    }
+}
+// superblock table: C[c] + the exclusive prefix of the superblock totals (already in `csb`)
+__global__ void kj_bld_csb_add_c(uint64_t* __restrict__ csb, uint64_t nsb, const uint64_t* __restrict__ Cdev, int alen) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nsb * KJ_CSB_STRIDE; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t c = (uint32_t)(i % KJ_CSB_STRIDE); if (c < (uint32_t)alen) csb[i] += Cdev[c];
+    }
+}
+
+// rows per chunk of the compact build (a whole number of superblocks); KJ_BUILD_CHUNK_ROWS: developer hook that forces many chunks on small indexes
+static uint64_t kj_compact_chunk_rows() {
+    uint64_t ch = 1ull << 30;
+    if (const char* e = getenv("KJ_BUILD_CHUNK_ROWS")) { const long long x = atoll(e); if (x > 0 && (x & ((1ll << KJ_CSB_SHIFT) - 1)) == 0) ch = (uint64_t)x; }
+    return ch;
+}
+// The compact layout's records and superblock table in one pass over the BWT: the raw bytes go up one chunk at a time (rep == 1), so the peak is
+// the final arrays plus one chunk; a scan over the per-superblock totals then gives the superblock table and C[].
+static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBuildLcode& lc, uint32_t rep, uint64_t& tot) {
+    KjHostIndex& H = c->H; const int alen = H.alen; const uint64_t n = H.bwtlen, nb = H.nb, nsb = kj_csb_count(n);
+    const uint64_t CH = kj_compact_chunk_rows(), sb_per_chunk = CH >> KJ_CSB_SHIFT;
+    int rc; KjDevBuf bwt, sbt, small;
+    if ((rc = c->rank.grow(nb * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
+    tot += nb * KJ_RANK_WORDS_COMPACT * 8 + nsb * KJ_CSB_STRIDE * 8;
+    if ((rc = sbt.grow(nsb * KJ_CSB_STRIDE * 4)) || (rc = small.grow(3 * KJ_MAX_ALEN * 8 + 64))) return rc;
+    uint64_t* d_tot = small.as<uint64_t>(); uint64_t* d_C = d_tot + KJ_MAX_ALEN + 1;
+    if (rep == 1) { if ((rc = bwt.grow((size_t)std::min(CH, n)))) return rc; }
+    else if ((rc = bwt.grow((size_t)v.bwtlen)) || (rc = kj_bld_upload(bwt.p, v.bwt, (size_t)v.bwtlen))) return rc;
+    for (uint64_t s0 = 0; s0 < nsb; s0 += sb_per_chunk) {
+        const uint64_t row0 = s0 << KJ_CSB_SHIFT, nsc = std::min(sb_per_chunk, nsb - s0);
+        if (rep == 1 && row0 < n) CK(cudaMemcpy(bwt.p, v.bwt + row0, (size_t)(std::min(n, row0 + CH) - row0), cudaMemcpyHostToDevice));
+        kj_bld_compact<<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, c->rank.as<uint64_t>(), sbt.as<uint32_t>());
+        CK(cudaGetLastError()); c->launches++;
+        if (rep == 1) CK(cudaDeviceSynchronize());          // the next chunk's upload overwrites the staging buffer
+    }
+    bwt.reset();
+    kj_bld_scan_tiles<<<1, 32 * KJ_MAX_ALEN>>>(sbt.as<uint32_t>(), nsb, c->letters.as<uint64_t>(), d_tot);
+    CK(cudaGetLastError());
+    uint64_t tots[KJ_MAX_ALEN]; CK(cudaMemcpy(tots, d_tot, sizeof tots, cudaMemcpyDeviceToHost));
+    H.C[0] = 0; for (int a = 0; a < alen; a++) H.C[a + 1] = H.C[a] + tots[a];
+    if (H.C[alen] != n) { kj_err() = "letter counts do not add up"; return KJ_ERR_IO; }
+    CK(cudaMemcpy(d_C, H.C, sizeof(uint64_t) * (size_t)(alen + 1), cudaMemcpyHostToDevice));
+    kj_bld_csb_add_c<<<c->sm_count * 4, 256>>>(c->letters.as<uint64_t>(), nsb, d_C, alen);
+    CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches += 2;
+    return KJ_OK;
+}
+
+// Layout of a 64-bit index built on the device: wide exactly when the peak HBM of the wide construction fits in the memory free now, else
+// compact; when the compact construction does not fit either, KJ_ERR_NOMEM before anything large is allocated.  A peak is the maximum over the
+// construction's phases: (1) BWT staging + scratch + the rank arrays, (2) rank arrays + suffix-array arrays + the upload chunk of the sampled
+// suffix array, (3) rank arrays + suffix-array arrays + the two level buffers of the k-mer table.
+static int kj_choose_layout(kj_ctx* c, const kj_index_view& v, uint32_t rep) {
+    KjHostIndex& H = c->H;
+    if (H.wide == KJ_LAYOUT_NARROW) return KJ_OK;
+    const uint64_t n = H.bwtlen, alen = (uint64_t)H.alen;
+    size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));
+    const uint64_t n_sa = rep == 1 ? (uint64_t)v.ncheck + 1 : (uint64_t)std::max<int64_t>((int64_t)((n - 1) >> H.sa_exp) - H.sa_bias + 1, 4);
+    const uint64_t acc = H.seq_acc.empty() ? 1 : 2;
+    const uint64_t sa = acc * (n_sa + (uint64_t)H.nseq) * 4, upload = rep == 1 ? std::min<uint64_t>(1ull << 26, n_sa) * (uint64_t)v.nbytes : 0;
+    uint64_t levels = 0;
+    { const char* ek = getenv("KJ_KMER_K"); const int k = ek ? atoi(ek) : kj_default_kmer_k(n);
+      if (k >= 2 && k <= 7 && alen == 21) { levels = 2 * sizeof(KjKmer); for (int d = 0; d < k; d++) levels *= 20; } }
+    auto peak = [&](uint64_t arrays, uint64_t build) { return std::max(std::max(arrays + build, arrays + sa + upload), arrays + sa + levels); };
+    const uint64_t nb_w = n / KJ_RANK_ROWS_WIDE + 1, ntiles = (nb_w + KJ_BLD_THREADS - 1) / KJ_BLD_THREADS;
+    const uint64_t wide_peak = peak(kj_rank_array_words(KJ_LAYOUT_WIDE, H.alen, nb_w) * 8 + kj_letters_words(KJ_LAYOUT_WIDE, n) * 8, (uint64_t)v.bwtlen + ntiles * KJ_MAX_ALEN * 12);
+    if (H.wide == KJ_LAYOUT_WIDE && wide_peak <= fr) return KJ_OK;
+    const uint64_t nb_c = n / KJ_RANK_ROWS_COMPACT + 1, nsb = kj_csb_count(n);
+    const uint64_t compact_peak = peak(kj_rank_array_words(KJ_LAYOUT_COMPACT, H.alen, nb_c) * 8 + kj_letters_words(KJ_LAYOUT_COMPACT, n) * 8,
+                                       nsb * KJ_CSB_STRIDE * 4 + (rep == 1 ? std::min(kj_compact_chunk_rows(), n) : (uint64_t)v.bwtlen));
+    if (compact_peak > fr) {
+        char b[256]; snprintf(b, sizeof b, "index of %llu rows does not fit in HBM: building it needs %llu bytes (compact layout), %llu bytes are free",
+                              (unsigned long long)n, (unsigned long long)compact_peak, (unsigned long long)fr);
+        kj_err() = b; return KJ_ERR_NOMEM;
+    }
+    H.wide = KJ_LAYOUT_COMPACT; H.nb = nb_c;
+    return KJ_OK;
+}
+
+// The one-hot layouts (narrow, wide): rank records and packed letters from the whole BWT on the device.
+static int kj_device_build_onehot(kj_ctx* c, const kj_index_view& v, const KjBuildLcode& lc, uint32_t rep, uint64_t& tot) {
     KjHostIndex& H = c->H; const int alen = H.alen; const uint64_t n = H.bwtlen, nb = H.nb; const int wide = H.wide;
     const uint32_t RB = kj_rank_rows(wide), RW = kj_rank_words(wide);
-    KjBuildLcode lc; memcpy(lc.v, lcode, 256);
     const int grid_big = c->sm_count * 16;
     // ---- BWT bytes to the device (freed again below)
     KjDevBuf bwt; int rc = bwt.grow((size_t)v.bwtlen); if (rc) return rc;
@@ -223,8 +344,17 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
     tot += nwords * 8;
     kj_bld_letters<<<grid_big, 256>>>(d_bwt, lc, n, rep, nwords, c->letters.as<uint64_t>());
     CK(cudaGetLastError()); CK(cudaDeviceSynchronize());
-    bwt.reset(); tc.reset(); tp.reset();      // before the suffix-array arrays are allocated
     c->launches += 4;
+    return KJ_OK;       // the BWT and tile arrays go before the suffix-array arrays are allocated
+}
+
+// Builds the large arrays of the context on the device.  c->H holds the meta data (kj_build_host_meta); `base` (scaled build only) is a
+// finished context over the same index with copies = 1, whose device index resolves base suffix-array rows to taxa.
+static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcode[256], uint32_t rep, const kj_ctx* base, uint64_t& tot) {
+    KjHostIndex& H = c->H; const uint64_t n = H.bwtlen; int rc;
+    KjBuildLcode lc; memcpy(lc.v, lcode, 256);
+    const int grid_big = c->sm_count * 16;
+    if ((rc = H.wide == KJ_LAYOUT_COMPACT ? kj_device_build_compact(c, v, lc, rep, tot) : kj_device_build_onehot(c, v, lc, rep, tot))) return rc;
     // ---- sequence -> taxon, sampled suffix array -> taxon
     if ((rc = upload(H.seq_tax, c->seq_tax, tot))) return rc;
     if (!H.seq_acc.empty()) {
@@ -258,7 +388,8 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
         n_sa = last >= 0 ? (uint64_t)last + 1 : 0;
         if ((rc = c->sa_tax.grow(std::max<size_t>(n_sa * 4, 16)))) return rc;
         tot += std::max<size_t>(n_sa * 4, 16);
-        if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        if (base->H.wide == KJ_LAYOUT_COMPACT) kj_bld_sa_tax_scaled<KjCompactIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        else if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else kj_bld_sa_tax_scaled<uint32_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches++;
     }
@@ -271,7 +402,8 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
 static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, int& k_out) {
     KjHostIndex& H = c->H; const int wide = H.wide; const KjDevIndex* ix = c->ix.as<KjDevIndex>();
     if (H.quirk_lo != ~0ull && &dst == &c->kmer) {
-        if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>()); else kj_bld_quirk<uint32_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        if (wide == KJ_LAYOUT_COMPACT) kj_bld_quirk<KjCompactIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        else if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>()); else kj_bld_quirk<uint32_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         CK(cudaGetLastError()); CK(cudaMemcpy(H.quirk_d, c->quirk.p, sizeof H.quirk_d, cudaMemcpyDeviceToHost)); c->launches++;
     }
     k_out = 0;
@@ -286,7 +418,8 @@ static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, 
     uint64_t n_cur = 20;
     for (int d = 1; d < k; d++) {
         const unsigned g = (unsigned)std::min<uint64_t>((n_cur * 20 + 255) / 256, (uint64_t)c->sm_count * 32);
-        if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>()); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        if (wide == KJ_LAYOUT_COMPACT) kj_bld_kmer_level<KjCompactIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        else if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>()); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         CK(cudaGetLastError()); c->launches++;
         std::swap(a, b); n_cur *= 20;
     }

@@ -133,14 +133,57 @@ static KJ_DEV IdxT kj_rank_at(const uint64_t* base, IdxT k) {
     const uint32_t add = wi == 0 ? 0u : ((uint32_t)(hdr >> (32u + 8u * wi)) & 0xffu);
     return (IdxT)((hdr & KJ_CNT_MASK) + (uint64_t)(add + pc));
 }
+// The compact layout (kj_layout.h) runs the 64-bit kernels with IdxT = KjCompactIdx: a 64-bit unsigned type distinct from uint64_t (unsigned
+// long), so that the layout is a compile-time property of the instantiation and the narrow and wide instantiations are untouched by it.
+typedef unsigned long long KjCompactIdx;
+template <class IdxT> struct KjIsCompact { static constexpr bool v = false; };
+template <> struct KjIsCompact<KjCompactIdx> { static constexpr bool v = true; };
+static_assert(sizeof(KjCompactIdx) == 8 && !KjIsCompact<uint64_t>::v, "KjCompactIdx must be a 64-bit type distinct from uint64_t");
+// compact layout: rank of letter c at row k from the plane words of k's half-record `pl` (5 independent loads, issued by the caller) plus the
+// midpoint count and the superblock count -- every address a function of (c, k) only, and no branch on the data
+static KJ_DEV uint64_t kj_crank_planes(const KjDevIndex& ix, const uint64_t* rec, const uint64_t pw[5], uint32_t c, uint64_t k) {
+    const uint64_t cw = kj_ld64(rec + KJ_CPT_COUNT_WORD + (c >> 2));
+    const uint64_t sb = kj_ld64(ix.csb + (size_t)(k >> KJ_CSB_SHIFT) * KJ_CSB_STRIDE + c);
+    uint64_t m = ~0ull;
+    #pragma unroll
+    for (int b = 0; b < 5; b++) m &= pw[b] ^ ((uint64_t)((c >> b) & 1u) - 1ull);      // rows whose letter equals c
+    const uint32_t h = (uint32_t)(k >> 6) & 1u;
+    const uint64_t below = (1ull << ((uint32_t)k & 63u)) - 1ull;
+    // second half: rows [midpoint, k) are added; first half: rows [k, midpoint) are subtracted
+    const uint64_t pc = (uint64_t)kj_popcll(m & (h ? below : ~below));
+    const uint64_t v = sb + ((cw >> (16u * (c & 3u))) & 0xffffull);
+    return h ? v + pc : v - pc;
+}
+static KJ_DEV const uint64_t* kj_crec(const KjDevIndex& ix, uint64_t k) { return ix.rank + (size_t)(k >> 7) * KJ_RANK_WORDS_COMPACT; }
+static KJ_DEV void kj_cplanes(const uint64_t* rec, uint64_t k, uint64_t pw[5]) {
+    const uint64_t* pl = rec + 5u * ((uint32_t)(k >> 6) & 1u);
+    #pragma unroll
+    for (int b = 0; b < 5; b++) pw[b] = kj_ld64(pl + b);
+}
+static KJ_DEV uint64_t kj_crank(const KjDevIndex& ix, uint32_t c, uint64_t k) {
+    const uint64_t* rec = kj_crec(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    return kj_crank_planes(ix, rec, pw, c, k);
+}
+// one LF step of the compact layout: the letter of row k and its rank, from k's record
+static KJ_DEV uint64_t kj_clf(const KjDevIndex& ix, uint64_t k, uint32_t& c) {
+    const uint64_t* rec = kj_crec(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    const uint32_t bit = (uint32_t)k & 63u; c = 0;
+    #pragma unroll
+    for (int b = 0; b < 5; b++) c |= (uint32_t)((pw[b] >> bit) & 1ull) << b;
+    return kj_crank_planes(ix, rec, pw, c, k);
+}
 static KJ_DEV const uint64_t* kj_letter_base(const KjDevIndex& ix, uint32_t c) { return ix.rank_base[c]; }
 template <class IdxT>
-static KJ_DEV IdxT kj_rank(const KjDevIndex& ix, uint32_t c, IdxT k) { return kj_rank_at<IdxT>(kj_letter_base(ix, c), k); }
+static KJ_DEV IdxT kj_rank(const KjDevIndex& ix, uint32_t c, IdxT k) {
+    if constexpr (KjIsCompact<IdxT>::v) return (IdxT)kj_crank(ix, c, (uint64_t)k);
+    else return kj_rank_at<IdxT>(kj_letter_base(ix, c), k);
+}
 // UpdateSI (bwt.c:160-173)
 template <class IdxT>
 static KJ_DEV bool kj_update_si(const KjDevIndex& ix, uint32_t c, IdxT& lo, IdxT& hi) {
-    const uint64_t* base = kj_letter_base(ix, c);
-    IdxT nlo = kj_rank_at<IdxT>(base, lo), nhi = kj_rank_at<IdxT>(base, hi);
+    IdxT nlo, nhi;
+    if constexpr (KjIsCompact<IdxT>::v) { nlo = (IdxT)kj_crank(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank(ix, c, (uint64_t)hi); }
+    else { const uint64_t* base = kj_letter_base(ix, c); nlo = kj_rank_at<IdxT>(base, lo); nhi = kj_rank_at<IdxT>(base, hi); }
     // the reference's checkpoint quirk (indexes with bwtlen = m * 2^16 only, kj_host.cpp): the last 129 positions rank lower by a per-letter
     // constant.  Such indexes are routed to the 64-bit kernels, so the 32-bit ones do not carry the test.
     if (sizeof(IdxT) == 8) { if (hi >= (IdxT)ix.quirk_lo) { const IdxT d = (IdxT)ix.quirk_d[c]; nhi -= d; if (lo >= (IdxT)ix.quirk_lo) nlo -= d; } }
@@ -167,7 +210,8 @@ static KJ_DEV uint64_t kj_sa_locate(const KjDevIndex& ix, uint64_t k, bool& is_s
     uint32_t c = 1;
     KJ_ROLLED
     while (c != 0 && (k & ix.sa_check)) {
-        c = kj_letter(ix, k); const bool q = k >= ix.quirk_lo; k = (uint64_t)kj_rank<IdxT>(ix, c, (IdxT)k); if (q) k -= ix.quirk_d[c];
+        if constexpr (KjIsCompact<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf(ix, k, c); if (q) k -= ix.quirk_d[c]; }
+        else { c = kj_letter(ix, k); const bool q = k >= ix.quirk_lo; k = (uint64_t)kj_rank<IdxT>(ix, c, (IdxT)k); if (q) k -= ix.quirk_d[c]; }
 #if defined(KJ_EMU)
         kj_emu_stats.sa_lf_steps++;
 #endif

@@ -150,9 +150,11 @@ static KjKernel kj_select_kernel_t(bool gws, bool fixed, bool verbose, int role)
     }
     return kj_classify_kernel<MODE, T, false, false, false, 0>;
 }
-static KjKernel kj_select_kernel(int mode, bool wide, bool gws, bool fixed, bool verbose, int role) {
-    if (mode == 0) return wide ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
-    return wide ? kj_select_kernel_t<1, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<1, uint32_t>(gws, fixed, verbose, role);
+// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact (64-bit intervals; kj_layout.h)
+static KjKernel kj_select_kernel(int mode, int layout, bool gws, bool fixed, bool verbose, int role) {
+    if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_kernel_t<0, KjCompactIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjCompactIdx>(gws, fixed, verbose, role);
+    if (mode == 0) return layout ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
+    return layout ? kj_select_kernel_t<1, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<1, uint32_t>(gws, fixed, verbose, role);
 }
 
 __global__ void kj_maxlen_kernel(const uint64_t* __restrict__ off, uint64_t n, unsigned int* __restrict__ out) {
@@ -225,7 +227,7 @@ struct kj_ctx {
     KjDevIndex dix{};              // host copy of the descriptor (device pointers inside)
     KjDevBuf ix, tables;
     KjDevBuf ix_mem, kmer_mem; int kmer_k_mem = 0;      // the MEM kernels' own descriptor: same index, 7-mer table (kj_create)
-    KjDevBuf rank, letters, sa_tax, seq_tax, sa_acc, seq_acc, tax_parent, tax_depth, tax_id, lnfact, kmer;
+    KjDevBuf rank, letters, sa_tax, seq_tax, sa_acc, seq_acc, tax_parent, tax_depth, tax_id, lnfact, kmer;    // compact layout: `letters` holds the superblock table
     KjDevBuf row_tax;              // taxon per BWT row (kj_device_build_row_tax; empty: the kernels walk)
     uint64_t index_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;
     // run state
@@ -320,7 +322,7 @@ static int upload_descriptor(kj_ctx* c) {
     KjHostIndex& H = c->H; KjDevIndex& D = c->dix; memset(&D, 0, sizeof D);
     D.rank = c->rank.as<const uint64_t>(); D.nb = H.nb; D.letters = c->letters.as<const uint64_t>(); D.bwtlen = H.bwtlen; D.alen = H.alen;
     for (int a = 0; a <= H.alen; a++) D.C[a] = H.C[a];
-    for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
+    if (H.wide != KJ_LAYOUT_COMPACT) for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
     D.sa_acc = c->sa_acc.as<const uint32_t>(); D.seq_acc = c->seq_acc.as<const uint32_t>();
     D.sa_tax = c->sa_tax.as<const uint32_t>(); D.seq_tax = c->seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
     D.n_sa = c->n_sa; D.row_tax = c->row_tax.as<const uint32_t>(); D.nseq = H.nseq;
@@ -389,6 +391,7 @@ static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, 
     std::unique_ptr<kj_ctx, void (*)(kj_ctx*)> guard(c, kj_destroy);
     const auto t0 = std::chrono::steady_clock::now();
     uint8_t lcode[256]; rc = kj_build_host_meta(v, t, copies, c->H, lcode); if (rc) return rc;
+    if ((rc = kj_choose_layout(c, v, copies))) return rc;
     uint64_t tot = 0;
     if ((rc = upload_small(c, tot)) || (rc = kj_device_build(c, v, lcode, copies, base, tot))) return rc;
     c->H.kmer_k = 0;
@@ -422,12 +425,12 @@ extern "C" int kj_create_scaled(kj_ctx** out, int device, const kj_params* param
     return rc;
 }
 extern "C" double kj_index_build_ms(const kj_ctx* c) { return c ? c->build_ms : 0.0; }
-// test hook: checksums of the index arrays as they sit in HBM (rank, letters, sa_tax, seq_tax, kmer), to compare the device construction
-// with the host transcoder array for array
+// test hook: checksums of the index arrays as they sit in HBM (rank, letters or the compact superblock table, sa_tax, seq_tax, kmer | bwtlen,
+// layout, n_sa), to compare the device construction with the host transcoder array for array
 extern "C" int kj_debug_index_checksums(kj_ctx* c, uint64_t out[8]) {
     if (!c || !out) return KJ_ERR_ARG; CK(cudaSetDevice(c->device)); CK(cudaDeviceSynchronize());
     const KjHostIndex& H = c->H; memset(out, 0, 64);
-    const size_t sz[5] = {(size_t)H.alen * H.nb * kj_rank_words(H.wide) * 8, (size_t)(H.bwtlen / KJ_LETTERS_PER_WORD + 2) * 8, (size_t)c->n_sa * 4, (size_t)H.nseq * 4,
+    const size_t sz[5] = {(size_t)kj_rank_array_words(H.wide, H.alen, H.nb) * 8, (size_t)kj_letters_words(H.wide, H.bwtlen) * 8, (size_t)c->n_sa * 4, (size_t)H.nseq * 4,
                           H.kmer_k ? (size_t)pow(20.0, H.kmer_k) * (H.wide ? sizeof(KjKmer) : sizeof(KjKmer32)) : 0};
     const void* ptr[5] = {c->rank.p, c->letters.p, c->sa_tax.p, c->seq_tax.p, c->kmer.p};
     for (int i = 0; i < 5; i++) { std::vector<uint8_t> h(sz[i]); if (sz[i]) CK(cudaMemcpy(h.data(), ptr[i], sz[i], cudaMemcpyDeviceToHost)); out[i] = kj_mix_bytes(0x6b616a75ull + i, h.data(), h.size()); }
@@ -729,6 +732,7 @@ extern "C" int kj_classify_verbose2(kj_ctx* c, const char* seq1, const uint64_t*
 }
 extern "C" uint64_t kj_kernel_launches(const kj_ctx* c) { return c ? c->launches : 0; }
 extern "C" uint64_t kj_index_bytes(const kj_ctx* c) { return c ? c->index_bytes : 0; }
+extern "C" int kj_index_layout(const kj_ctx* c) { return c ? c->H.wide : -1; }
 extern "C" double kj_last_kernel_ms(const kj_ctx* c) {
     if (!c) return 0.0;
     float ms = 0.f; if (cudaEventSynchronize(c->ev_b) != cudaSuccess) return 0.0;

@@ -206,8 +206,10 @@ int kj_build_host_meta(const kj_index_view& v, const kj_taxonomy_view& t, uint32
     }
     // KJ_FORCE_WIDE: exercise the 64-bit kernels on small test indexes.  Indexes with the reference's checkpoint quirk (below) also
     // take the 64-bit kernels: only those carry the rank correction, so that ordinary indexes pay nothing for the 1-in-65536 case.
+    // KJ_FORCE_COMPACT: the compact layout (kj_layout.h) for any index, to test it on small ones; otherwise it is chosen on the device when the
+    // wide construction does not fit in HBM (kj_choose_layout).
     const bool quirk = (n & 65535ull) == 0 && n >= 131072ull;
-    H.wide = (n >= 0xffffff00ull || getenv("KJ_FORCE_WIDE") || quirk) ? 1 : 0;
+    H.wide = getenv("KJ_FORCE_COMPACT") ? KJ_LAYOUT_COMPACT : (n >= 0xffffff00ull || getenv("KJ_FORCE_WIDE") || quirk) ? KJ_LAYOUT_WIDE : KJ_LAYOUT_NARROW;
     H.nb = n / kj_rank_rows(H.wide) + 1;
     // The reference's checkpoint quirk (fmicommon.h:60-73, 88-89, 114-158; pinned against the reference's own FMindex/get_suffix and CLI in
     // tests/test_oracle_vs_ref.py::test_bwtlen_multiple_of_65536):
@@ -288,9 +290,32 @@ int kj_build_host_index(const kj_index_view& v, const kj_taxonomy_view& t, KjHos
     const uint64_t* total = &ccount[(size_t)nch * alen];
     H.C[0] = 0; for (int a = 0; a < alen; a++) H.C[a + 1] = H.C[a] + total[a];
     if (H.C[alen] != n) { kj_err() = "letter counts do not add up"; return KJ_ERR_IO; }
-    try { H.rank.assign((size_t)alen * nb * RW, 0ull); H.letters.assign((size_t)(n / KJ_LETTERS_PER_WORD + 2), 0); }
+    try { H.rank.assign((size_t)kj_rank_array_words(H.wide, alen, nb), 0ull); H.letters.assign((size_t)kj_letters_words(H.wide, n), 0); }
     catch (...) { kj_err() = "out of host memory building the rank table"; return KJ_ERR_NOMEM; }
-    par([&](uint64_t c) {
+    if (H.wide == KJ_LAYOUT_COMPACT) {
+        // records: 5 bit-planes per 64-row half + the counts from the superblock start to the record's midpoint; then the superblock table
+        const uint64_t nsb = kj_csb_count(n); std::vector<uint64_t> sbt((size_t)nsb * KJ_CSB_STRIDE, 0);
+        std::vector<std::thread> th;
+        for (unsigned tI = 0; tI < nthr; tI++) th.emplace_back([&, tI] {
+            for (uint64_t sb = tI; sb < nsb; sb += nthr) {
+                uint64_t cnt[KJ_CSB_STRIDE] = {0};
+                for (uint64_t b = sb << (KJ_CSB_SHIFT - 7); b < nb && b < (sb + 1) << (KJ_CSB_SHIFT - 7); b++) {
+                    uint64_t* R = &H.rank[(size_t)b * KJ_RANK_WORDS_COMPACT];
+                    for (uint32_t i = 0; i < 128; i++) {
+                        if (i == 64) for (int a = 0; a < KJ_CSB_STRIDE; a++) ((uint16_t*)(R + KJ_CPT_COUNT_WORD))[a] = (uint16_t)cnt[a];
+                        const uint64_t k = b * 128 + i; const uint32_t l = k < n ? lcode[v.bwt[k]] : 31u;
+                        if (k < n) cnt[l]++;
+                        for (int bit = 0; bit < 5; bit++) R[5 * (i >> 6) + bit] |= (uint64_t)((l >> bit) & 1u) << (i & 63);
+                    }
+                }
+                for (int a = 0; a < KJ_CSB_STRIDE; a++) sbt[(size_t)sb * KJ_CSB_STRIDE + a] = cnt[a];
+            }
+        });
+        for (auto& x : th) x.join();
+        uint64_t run[KJ_CSB_STRIDE] = {0};
+        for (uint64_t sb = 0; sb < nsb; sb++) for (int a = 0; a < KJ_CSB_STRIDE; a++) {
+            H.letters[(size_t)sb * KJ_CSB_STRIDE + a] = (a < alen ? H.C[a] : 0) + run[a]; run[a] += sbt[(size_t)sb * KJ_CSB_STRIDE + a]; }
+    } else par([&](uint64_t c) {
         uint64_t run[KJ_MAX_ALEN]; for (int a = 0; a < alen; a++) run[a] = H.C[a] + ccount[(size_t)c * alen + a];
         uint64_t e = std::min(n, (c + 1) * CH);
         for (uint64_t b0 = c * CH; b0 < e; b0 += RB) {
@@ -305,8 +330,8 @@ int kj_build_host_index(const kj_index_view& v, const kj_taxonomy_view& t, KjHos
         for (uint64_t k = c * CH; k < e; k++) H.letters[k / KJ_LETTERS_PER_WORD] |= (uint64_t)lcode[v.bwt[k]] << (5 * (k % KJ_LETTERS_PER_WORD));
     });
     // the record after the last letter (k == bwtlen lands there when bwtlen % RB == 0; otherwise the last partial block already exists)
-    if (n % RB == 0) for (int a = 0; a < alen; a++) H.rank[((size_t)a * nb + (nb - 1)) * RW] = H.C[a] + total[a];
-    if (H.wide) {   // fold the in-block prefix popcounts into the header
+    if (n % RB == 0 && H.wide != KJ_LAYOUT_COMPACT) for (int a = 0; a < alen; a++) H.rank[((size_t)a * nb + (nb - 1)) * RW] = H.C[a] + total[a];
+    if (H.wide == KJ_LAYOUT_WIDE) {   // fold the in-block prefix popcounts into the header
         std::vector<std::thread> th; const size_t tot = (size_t)alen * nb;
         for (unsigned tI = 0; tI < nthr; tI++) th.emplace_back([&, tI] { for (size_t i = tI; i < tot; i += nthr) { uint64_t* B = &H.rank[i * 4];
             uint64_t p1 = (uint64_t)__builtin_popcountll(B[1]), p2 = p1 + (uint64_t)__builtin_popcountll(B[2]); B[0] = (B[0] & KJ_CNT_MASK) | (p1 << KJ_P1_SHIFT) | (p2 << KJ_P2_SHIFT); } });
@@ -338,6 +363,14 @@ int kj_build_host_index(const kj_index_view& v, const kj_taxonomy_view& t, KjHos
 
 // host-side rank on the device layout (used only to fill the k-mer table)
 static inline uint64_t host_rank(const KjHostIndex& H, uint32_t c, uint64_t k) {
+    if (H.wide == KJ_LAYOUT_COMPACT) {
+        const uint64_t* R = &H.rank[(size_t)(k >> 7) * KJ_RANK_WORDS_COMPACT]; const uint32_t h = (uint32_t)(k >> 6) & 1u, bit = (uint32_t)k & 63u;
+        uint64_t m = ~0ull; for (int b = 0; b < 5; b++) m &= ((c >> b) & 1u) ? R[5 * h + b] : ~R[5 * h + b];
+        const uint64_t below = (1ull << bit) - 1ull;
+        const uint64_t mid = H.letters[(size_t)(k >> KJ_CSB_SHIFT) * KJ_CSB_STRIDE + c] + ((const uint16_t*)(R + KJ_CPT_COUNT_WORD))[c];
+        const uint64_t v = h ? mid + (uint64_t)__builtin_popcountll(m & below) : mid - (uint64_t)__builtin_popcountll(m & ~below);
+        return k >= H.quirk_lo ? v - H.quirk_d[c] : v;
+    }
     const uint32_t RB = kj_rank_rows(H.wide), RW = kj_rank_words(H.wide);
     uint64_t b = k / RB; uint32_t r = (uint32_t)(k - b * RB); const uint64_t* B = &H.rank[((size_t)c * H.nb + b) * RW];
     uint32_t wi = r >> 6, bit = r & 63u; uint64_t ww = B[1 + wi];
@@ -345,6 +378,7 @@ static inline uint64_t host_rank(const KjHostIndex& H, uint32_t c, uint64_t k) {
     const uint64_t v = (H.wide ? (B[0] & KJ_CNT_MASK) : B[0]) + add + (uint64_t)__builtin_popcountll(ww & ((1ull << bit) - 1ull));
     return k >= H.quirk_lo ? v - H.quirk_d[c] : v;                  // the reference's checkpoint quirk (kj_build_host_index)
 }
+uint64_t kj_host_rank(const KjHostIndex& H, uint32_t c, uint64_t k) { return host_rank(H, c, k); }
 // index = a0*20^(k-1) + a1*20^(k-2) + ... + a(k-1), a_t = letter consumed t-th by the backward search (end of the k-mer first), letters 1..20 -> 0..19
 void kj_build_kmer_table(KjHostIndex& H, int k) {
     H.kmer.clear(); H.kmer32.clear(); H.kmer_k = 0;
@@ -451,6 +485,7 @@ template <class T> bool get(FILE* f, std::vector<T>& v, uint64_t n) { v.resize((
 }  // namespace
 
 int kj_host_index_write(const KjHostIndex& H, const char* path) {
+    if (H.wide == KJ_LAYOUT_COMPACT) { kj_err() = "device-native index files hold the narrow and wide layouts only"; return KJ_ERR_UNSUPPORTED; }
     FILE* f = fopen(path, "wb"); if (!f) { kj_err() = std::string("Could not open file ") + path + " for writing"; return KJ_ERR_IO; }
     NativeHeader h; memset(&h, 0, sizeof h);
     h.version = kNativeVersion; h.sizeof_tables = (uint32_t)sizeof(KjTables); h.sizeof_rank = 8u * kj_rank_words(H.wide); h.alen = (uint32_t)H.alen;

@@ -38,6 +38,8 @@ uint64_t kj_mix_bytes(uint64_t h, const void* p, size_t n);   // order-sensitive
 int kj_build_host_index(const kj_index_view& v, const kj_taxonomy_view& t, KjHostIndex& out);
 // the small / BWT-independent part only (the large arrays are then built on the device, kj_build.h); lcode = byte code -> letter
 int kj_build_host_meta(const kj_index_view& v, const kj_taxonomy_view& t, uint32_t copies, KjHostIndex& out, uint8_t lcode[256]);
+// FMindex(c, k) on the transcoder's arrays (any layout, the checkpoint quirk applied): the CPU reference of the device rank query
+uint64_t kj_host_rank(const KjHostIndex& H, uint32_t c, uint64_t k);
 // SA intervals of all 20^k k-mers over the 20 residue letters (exactness-preserving shortcut for the first k LF steps)
 void kj_build_kmer_table(KjHostIndex& H, int k);
 // k of the k-mer interval table: 6 letters (20^6 entries, 0.5-1 GB) once the index is large enough that 6-mers are mostly present

@@ -6,7 +6,7 @@
 // ~18-30 bytes.  Rank values are a pure function of the decoded letters (SURVEY.md 8a exactness note a),
 // so the device uses its own layout, built at load time from the decoded letters:
 //
-//   rank[c][b] : one record per (letter c, block b of 64 or 192 BWT positions; two layouts, below); the 192-row one:
+//   rank[c][b] : one record per (letter c, block b of 64 or 192 BWT positions; one-hot layouts, below); the 192-row one:
 //                { hdr = C[c] + #{p < 192 b : L[p] == c} (40 bit) + the popcounts of w0 and w0|w1 (2 x 8 bit),
 //                  w0,w1,w2 = one-hot bitmap of L[p]==c }
 //                -> FMindex(c,k) touches exactly ONE 32-byte DRAM sector and needs ONE 64-bit popcount.
@@ -21,18 +21,38 @@
 #pragma once
 #include <stdint.h>
 
-// Two record layouts, chosen per index at load time:
+// Three record layouts, chosen per index at load time:
 //   narrow (bwtlen < 2^32, 32-bit interval kernels): 16-byte records per 64 rows  { hdr = C[c] + #c before the block, w0 = one-hot bitmap }
 //          -> one 16-byte load + one popcount per rank query, no division; 5.25 B per BWT row (faster than the 192-row layout where both fit)
 //   wide   (bwtlen >= 2^32, 64-bit interval kernels): 32-byte records per 192 rows { hdr (40-bit count | popc(w0) | popc(w0)+popc(w1)), w0, w1, w2 }
 //          -> 3.5 B per row: an index of 1.2e10 rows takes 42 GB of the 80 GB HBM instead of 63 GB
+//   compact (64-bit kernels, indexes whose wide construction does not fit in HBM): the letters themselves, not one bitmap per letter.
+//          128-byte records per 128 rows { 5 bit-planes of rows 0-63 | 5 bit-planes of rows 64-127 (2 x 40 B) | 24 x uint16: #c from the start
+//          of the record's 65536-row superblock to the record's midpoint (row 64) }, plus `csb` = C[c] + #c before each superblock (24 x uint64
+//          per superblock).  FMindex(c,k) = csb + mid count +/- the popcount of "plane word == c" between k and the midpoint: 5 plane words, one
+//          count word and one superblock word, all addressed from (c,k) alone.  The same record gives the letter of row k (no `letters` array).
+//          1.003 B per row: refseq_ref (2.7e10 rows) fits an 80 GB H100.  Rows past bwtlen hold letter 31, which no rank query counts.
+// Layout codes (KjDevIndex::wide, KjHostIndex::wide): 0 narrow, 1 wide, 2 compact.
+#define KJ_LAYOUT_NARROW 0
+#define KJ_LAYOUT_WIDE 1
+#define KJ_LAYOUT_COMPACT 2
 #define KJ_RANK_ROWS_NARROW 64
 #define KJ_RANK_ROWS_WIDE 192
+#define KJ_RANK_ROWS_COMPACT 128
 #define KJ_RANK_WORDS_NARROW 2
 #define KJ_RANK_WORDS_WIDE 4
-static inline uint32_t kj_rank_rows(int wide) { return wide ? KJ_RANK_ROWS_WIDE : KJ_RANK_ROWS_NARROW; }
-static inline uint32_t kj_rank_words(int wide) { return wide ? KJ_RANK_WORDS_WIDE : KJ_RANK_WORDS_NARROW; }
+#define KJ_RANK_WORDS_COMPACT 16
+#define KJ_CPT_COUNT_WORD 10       // compact record: the 16-bit midpoint counts start at word 10
+#define KJ_CSB_SHIFT 16            // compact superblock: 2^16 rows = 512 records
+#define KJ_CSB_STRIDE 24           // compact superblock table: words per superblock (KJ_MAX_ALEN)
+static inline uint32_t kj_rank_rows(int layout) { return layout == KJ_LAYOUT_COMPACT ? KJ_RANK_ROWS_COMPACT : layout ? KJ_RANK_ROWS_WIDE : KJ_RANK_ROWS_NARROW; }
+static inline uint32_t kj_rank_words(int layout) { return layout == KJ_LAYOUT_COMPACT ? KJ_RANK_WORDS_COMPACT : layout ? KJ_RANK_WORDS_WIDE : KJ_RANK_WORDS_NARROW; }
+// 64-bit words of the rank array: one record per (letter, block) in the one-hot layouts, one record per block in the compact one
+static inline uint64_t kj_rank_array_words(int layout, int alen, uint64_t nb) { return (layout == KJ_LAYOUT_COMPACT ? 1ull : (uint64_t)alen) * nb * kj_rank_words(layout); }
+static inline uint64_t kj_csb_count(uint64_t bwtlen) { return (bwtlen >> KJ_CSB_SHIFT) + 1; }     // superblocks of a compact index (k = bwtlen included)
 #define KJ_LETTERS_PER_WORD 12
+// 64-bit words of the `letters` array: the packed letters, or the superblock table of the compact layout
+static inline uint64_t kj_letters_words(int layout, uint64_t bwtlen) { return layout == KJ_LAYOUT_COMPACT ? kj_csb_count(bwtlen) * KJ_CSB_STRIDE : bwtlen / KJ_LETTERS_PER_WORD + 2; }
 #define KJ_MAX_ALEN 24
 #define KJ_MAX_IDS 21              // max_match_ids = 20 -> the set holds at most 21 (ConsumerThread.cpp:805)
 #define KJ_MAX_BEST_SI 20          // max_matches_SI (Config.hpp:35)
@@ -61,9 +81,12 @@ struct KjTables {
 
 // (the 32-bit members are paired so that the descriptor has no padding holes: the kernels stage it in shared memory next to the work spaces)
 struct KjDevIndex {
-    const uint64_t* rank; uint64_t nb;          // [alen][nb] records of 2 (narrow) or 4 (wide) 64-bit words
-    const uint64_t* rank_base[KJ_MAX_ALEN];     // records of letter c (saves the multiply in the inner loop)
-    const uint64_t* letters;
+    const uint64_t* rank; uint64_t nb;          // [alen][nb] records of 2 (narrow) or 4 (wide) 64-bit words; compact: [nb] records of 16 words
+    const uint64_t* rank_base[KJ_MAX_ALEN];     // records of letter c (saves the multiply in the inner loop; not used by the compact layout)
+    union {
+        const uint64_t* letters;                // narrow, wide: the packed letters
+        const uint64_t* csb;                    // compact: [superblock][KJ_CSB_STRIDE] C[c] + #c before the superblock
+    };
     uint64_t bwtlen; int alen; uint32_t nseq;
     uint64_t C[KJ_MAX_ALEN + 1];                // C[c] = first SA row of letter c; C[alen] = bwtlen
     const uint32_t* sa_tax; const uint32_t* seq_tax;
@@ -73,7 +96,7 @@ struct KjDevIndex {
     const uint32_t* tax_parent; const uint32_t* tax_depth; const uint64_t* tax_id; uint32_t n_tax; int n_lnfact;
     const double* lnfact;
     const void* kmer; int kmer_k;               // direct-address table of k-mer intervals (KjKmer32 if !wide else KjKmer; 0 = off)
-    int wide;                                   // 1 if bwtlen >= 2^32 (64-bit interval arithmetic in the kernels)
+    int wide;                                   // layout code: 0 narrow (32-bit interval kernels), 1 wide, 2 compact (64-bit interval kernels)
     int mono;                                   // 1: true FM index (match starts monotone in the end position); 0: the reference's checkpoint quirk applies (no chain bounds)
     uint64_t quirk_lo; const uint64_t* quirk_d;         // rows k >= quirk_lo: FMindex(c,k) -= quirk_d[c] (reference checkpoint quirk, ~0 = none; [KJ_MAX_ALEN] in global memory)
     const KjTables* tables;
