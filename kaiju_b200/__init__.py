@@ -13,6 +13,8 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KJ_B200_LIB") or os.path.join(_HERE, "libkaijub200.so")   # KJ_B200_LIB: A/B builds of the same library
+MAX_READ_LEN = 16383           # default read-length limit, bases per mate (include/kaiju_b200.h KJ_MAX_READ_LEN)
+MAX_LONG_READ_LEN = 1048575     # the highest limit Classifier.set_max_read_len accepts (KJ_MAX_LONG_READ_LEN)
 
 MEM, GREEDY = 0, 1
 
@@ -75,6 +77,7 @@ def lib():
         L.kj_native_index_write.argtypes = [C.POINTER(KjIndexView), C.POINTER(KjTaxonomyView), C.c_char_p]
         L.kj_create_from_native.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(KjParams), C.c_char_p]
         L.kj_set_params.argtypes = [C.c_void_p, C.POINTER(KjParams)]
+        L.kj_set_max_read_len.argtypes = [C.c_void_p, C.c_uint32]
         L.kj_destroy.argtypes = [C.c_void_p]
         L.kj_classify.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
         L.kj_classify_verbose.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -181,8 +184,17 @@ class Classifier:
     """One GPU context: the .fmi index and nodes.dmp taxonomy resident in HBM + run parameters.
     `Classifier(native_path, None)` loads a device-native index file written by write_native_index()."""
 
-    def __init__(self, fmi_path, nodes_path, device=0, params=None, copies=1, **kw):
-        """copies > 1: the index of the collection in which every sequence occurs `copies` times (kj_create_scaled)."""
+    def __init__(self, fmi_path, nodes_path, device=0, params=None, copies=1, max_read_len=None, **kw):
+        """copies > 1: the index of the collection in which every sequence occurs `copies` times (kj_create_scaled).
+        max_read_len: admit mates of up to this many bases (see set_max_read_len); None keeps the default, MAX_READ_LEN."""
+        self._init(fmi_path, nodes_path, device, params, copies, **kw)
+        if max_read_len is not None:
+            try:
+                self.set_max_read_len(max_read_len)
+            except Exception:
+                self.close(); raise
+
+    def _init(self, fmi_path, nodes_path, device, params, copies, **kw):
         L = lib()
         self._ctx = C.c_void_p()
         if nodes_path is None:
@@ -209,6 +221,11 @@ class Classifier:
         finally:
             L.kj_fmi_free(fmi)
         self.device = device
+
+    def set_max_read_len(self, bases):
+        """Longest mate admitted, in bases (protein reads: bases // 3 residues), from MAX_READ_LEN (the default) to MAX_LONG_READ_LEN
+        (kj_set_max_read_len).  Longer reads make a classify call fail; mates above MAX_READ_LEN run the long-read kernels."""
+        _check(lib().kj_set_max_read_len(self._ctx, int(bases)))
 
     def set_params(self, params=None, **kw):
         self.params = params if params is not None else make_params(**kw)

@@ -23,6 +23,13 @@
 #define KJ_SEG_CAP(max_frag) ((max_frag) / 4u + 8u)
 struct KjKept { uint64_t lo; uint32_t len; uint32_t aux; };     // one suffix interval (an SI of bwt.h:25-34)
 
+// Field width is a compile-time property of an instantiation.  LONG = false: the kernels of mates up to KJ_MAX_READ_LEN bases (15-bit array
+// positions and 14-bit lengths in 32-bit queue payloads, 16-bit match positions, prefix sums and SEG counts).  LONG = true: the long-read
+// kernels (mates up to KJ_MAX_LONG_READ_LEN = 2^20 - 1 bases): 64-bit payloads, 32-bit positions, prefix sums and counts, unclamped scores.
+template <bool LONG> struct KjW { typedef uint32_t pay; typedef uint16_t pos; };
+template <> struct KjW<true> { typedef uint64_t pay; typedef uint32_t pos; };
+#define KJ_LONG_LO_BITS 40      // long kernels: suffix-array rows stay below 2^40, so a match start rides in the bits above (Greedy's result list)
+
 // (member order: the kernels read these from the parameter bank in 8-byte pairs; accs_off and total are read together)
 struct KjSmemLayout {
     uint32_t qkey_off, qpay_off, kept_off, res_off, res2_off, pre_off, ids_off, qord_off, aa_off, aa_stride, frag_off, hflag_off,
@@ -37,7 +44,9 @@ struct KjSmemLayout {
 #define KJ_GUARD(L, o)
 #endif
 static KJ_HD uint32_t kj_align(uint32_t x, uint32_t a) { return (x + a - 1) / a * a; }
+template <bool LONG = false>
 static KJ_HD KjSmemLayout kj_smem_layout(const KjRunParams& p) {
+    constexpr uint32_t pay_bytes = sizeof(typename KjW<LONG>::pay), match_bytes = LONG ? 24u : 16u, pre_bytes = sizeof(typename KjW<LONG>::pos);
     KjSmemLayout L; uint32_t o = 0;
 #if defined(KJ_EMU)
     L.nguard = 0;
@@ -45,7 +54,7 @@ static KJ_HD KjSmemLayout kj_smem_layout(const KjRunParams& p) {
     L.qkey_off = o; o += 8u * p.item_cap; KJ_GUARD(L, o)
     L.kept_off = o; o += 16u * p.kept_cap_smem; KJ_GUARD(L, o)
     L.segs_off = o; o += 8u * KJ_SEG_CAP(p.max_frag); KJ_GUARD(L, o)          // {int begin,end}
-    L.qpay_off = o; o += 4u * kj_align(p.item_cap, 2); KJ_GUARD(L, o)
+    L.qpay_off = o; o += pay_bytes * kj_align(p.item_cap, 2); KJ_GUARD(L, o)
     L.qord_off = o; o += kj_align(p.item_cap, 8); KJ_GUARD(L, o)           // slots in pop order (valid while no SEG piece was pushed)
     L.ids_off = o; o += 4u * 24u; KJ_GUARD(L, o)
     L.accs_off = o; o += 4u * 24u; KJ_GUARD(L, o)                            // accession ranks of the visited sequences (verbose output) + their count
@@ -57,15 +66,15 @@ static KJ_HD KjSmemLayout kj_smem_layout(const KjRunParams& p) {
     const uint32_t u = o;
     L.segcnt_off = u; L.seghist_off = u + 20u * 32u;
     // count histograms of the lane-parallel trim search for regions <= 127 residues; longer regions use the sorted-composition
-    // variant (kj_seg_trim_long), whose per-lane state (20 x {uint16 count, letter, position}) fits in the same bytes
+    // variant (kj_seg_trim_long), whose per-lane state (20 x {uint16 count, letter, position}; uint32 counts in the long kernels) fits in the same bytes
     const uint32_t seg_rows = p.max_frag + 2 < 130u ? p.max_frag + 2 : 130u;
     const uint32_t seg_bytes = 20u * 32u + kj_align(seg_rows * 32u, 8);
     uint32_t g_bytes = 0;
     L.res_off = u; L.res2_off = u; L.pre_off = u;
     if (p.mode == 1) {
-        L.res_off = u; g_bytes += 16u * kj_align(p.max_frag + 1, 2);           // per-j chain results
-        L.res2_off = u + g_bytes; g_bytes += 16u * kj_align(p.max_frag + 1, 2);  // recorded matches in class order
-        L.pre_off = u + g_bytes; g_bytes += 2u * kj_align(p.max_frag + 2, 4);    // prefix sums of the BLOSUM62 diagonal
+        L.res_off = u; g_bytes += match_bytes * kj_align(p.max_frag + 1, 2);           // per-j chain results
+        L.res2_off = u + g_bytes; g_bytes += match_bytes * kj_align(p.max_frag + 1, 2);  // recorded matches in class order
+        L.pre_off = u + g_bytes; g_bytes += pre_bytes * kj_align(p.max_frag + 2, 4);    // prefix sums of the BLOSUM62 diagonal
     }
     o = u + (seg_bytes > g_bytes ? seg_bytes : g_bytes);
     KJ_GUARD(L, o)
@@ -198,9 +207,10 @@ static KJ_DEV uint32_t kj_letter(const KjDevIndex& ix, uint64_t k) {
 #if defined(KJ_EMU)
 // emulator counters.  Phase A/B: rounds, round_steps (max over lanes, summed), lane_steps, chains, blocks, lookaheads; Greedy queue: pops_frag,
 // pops_var, var_steps, var_pushed; taxon look-up of the kept rows (kj_ids_and_lca_fn): id_reads (reads that got there), kept (their kept
-// intervals), sa_waves (waves of up to 32 rows), sa_lf_steps (LF steps summed over lanes), sa_dep_steps (max over the lanes of a wave, summed)
+// intervals), sa_waves (waves of up to 32 rows), sa_lf_steps (LF steps summed over lanes), sa_dep_steps (max over the lanes of a wave, summed);
+// long-read queue: lq_tops (look-ups of the top entry), lq_slots (queue slots they read: the sorted head plus the late entries scanned)
 struct KjEmuStats { unsigned long long rounds, round_steps, lane_steps, chains, blocks, lookaheads, pops_frag, pops_var, var_steps, var_pushed,
-                                       id_reads, kept, sa_waves, sa_lf_steps, sa_dep_steps; };
+                                       id_reads, kept, sa_waves, sa_lf_steps, sa_dep_steps, lq_tops, lq_slots; };
 extern thread_local KjEmuStats kj_emu_stats;
 #endif
 // get_suffix (bwt.c:105-121) reduced to the taxon of the sequence the suffix lies in
@@ -336,23 +346,109 @@ static KJ_DEV uint32_t kj_prefix_min_excl(const Warp& w, uint32_t v, uint32_t in
 // arr(2) segchecked(1) start(15) len(14).  Originals get order = arr<<16 | scan position (their
 // insertion order, ConsumerThread.cpp:196-268); SEG pieces and greedy variants take a running counter.
 // ---------------------------------------------------------------------------------------------
+// Long kernels: key64 = val<<40 | (0xffffffff-order)<<8 | 1 (a score is below 2^22); payload = arr(2) segchecked(1) . start(21 of the high
+// word) | len(32); originals get order = arr<<22 | scan position, so late entries start at 2^24.
 #define KJ_ORDER_LATE (1u << 20)
-struct KjQueue { uint64_t* key; uint32_t* pay; uint8_t* ord; uint32_t cap, n, late, next, nsorted; bool dirty; };    // scalars: uniform
-static KJ_DEV uint64_t kj_qkey(uint32_t val, uint32_t order) { return ((uint64_t)val << 32) | ((uint64_t)(0xffffffu - order) << 8) | 1ull; }
-static KJ_DEV uint32_t kj_qpay(uint32_t arr, bool segchecked, uint32_t start, uint32_t len) { return (arr << 30) | ((segchecked ? 1u : 0u) << 29) | (start << 14) | len; }
+#define KJ_ORDER_LATE_LONG (1u << 24)
+template <bool LONG = false>
+struct KjQueue { uint64_t* key; typename KjW<LONG>::pay* pay; uint8_t* ord; uint32_t cap, n, late, next, nsorted; bool dirty; };    // scalars: uniform
+template <bool LONG = false>
+static KJ_DEV uint64_t kj_qkey(uint32_t val, uint32_t order) {
+    if constexpr (LONG) return ((uint64_t)val << 40) | ((uint64_t)(0xffffffffu - order) << 8) | 1ull;
+    else return ((uint64_t)val << 32) | ((uint64_t)(0xffffffu - order) << 8) | 1ull;
+}
+template <bool LONG = false>
+static KJ_DEV uint32_t kj_qval(uint64_t key) { return (uint32_t)(key >> (LONG ? 40 : 32)); }
+template <bool LONG = false>
+static KJ_DEV typename KjW<LONG>::pay kj_qpay(uint32_t arr, bool segchecked, uint32_t start, uint32_t len) {
+    if constexpr (LONG) return ((uint64_t)((arr << 30) | ((segchecked ? 1u : 0u) << 29) | start) << 32) | len;
+    else return (arr << 30) | ((segchecked ? 1u : 0u) << 29) | (start << 14) | len;
+}
+template <bool LONG>
+static KJ_DEV void kj_qpay_dec(typename KjW<LONG>::pay p, uint32_t& arr, bool& segchecked, uint32_t& start, uint32_t& len) {
+    if constexpr (LONG) { const uint32_t hi = (uint32_t)((uint64_t)p >> 32); arr = hi >> 30; segchecked = (hi >> 29) & 1u; start = hi & 0x1fffffffu; len = (uint32_t)p; }
+    else { arr = p >> 30; segchecked = (p >> 29) & 1u; start = (p >> 14) & 0x7fffu; len = p & 0x3fffu; }
+}
+// long kernels: insertion order of a fragment of array a, closed by the stop before scan position pos (< 2^21) or the leftover of a frame
+static KJ_DEV uint32_t kj_frag_order_long(uint32_t a, bool leftover, uint32_t frame, uint32_t pos) { return (a << 22) | (leftover ? (1u << 21) + frame : pos); }
 
 // emit from several lanes at once (emit predicate per lane)
-static KJ_DEV void kj_queue_emit(KjWarpCtx& cx, KjQueue& q, bool emit, uint32_t val, uint32_t order, uint32_t pay) {
+template <bool LONG = false>
+static KJ_DEV void kj_queue_emit(KjWarpCtx& cx, KjQueue<LONG>& q, bool emit, uint32_t val, uint32_t order, typename KjW<LONG>::pay pay) {
     uint32_t mask = cx.w.ballot(emit);
     if (!mask) return;
     uint32_t cnt = (uint32_t)kj_popc(mask);
     if (q.n + cnt > q.cap) { if (cx.w.lane == 0) kj_flag_error(cx, 1u); return; }
-    if (emit) { uint32_t s = q.n + (uint32_t)kj_popc(mask & lanemask_lt(cx.w.lane)); q.key[s] = kj_qkey(val, order); q.pay[s] = pay; }
+    if (emit) { uint32_t s = q.n + (uint32_t)kj_popc(mask & lanemask_lt(cx.w.lane)); q.key[s] = kj_qkey<LONG>(val, order); q.pay[s] = pay; }
     q.n += cnt;
+}
+// Long kernels: the fragments of a long read (tens of thousands) are sorted once, keys and payloads together, by a warp bitonic sort in the work
+// space: O(n log^2 n / 32) steps, and every comparator takes the larger key to the lower index, so the missing elements of the next power of two
+// act as zero keys at the end and their comparators are skipped.  Afterwards [0, nsorted) is in pop order; entries pushed later (SEG pieces,
+// KJ_ORDER_LATE_LONG and above) are appended behind it and found by a scan over the live late entries only (kj_queue_top_long; a popped one is
+// replaced by the last).
+static KJ_DEV void kj_queue_rank_long(KjWarpCtx& cx, KjQueue<true>& q) {
+    cx.w.sync();
+    const uint32_t n = q.n; uint32_t np = 1; while (np < n) np <<= 1;
+    KJ_ROLLED
+    for (uint32_t k = 2; k <= np; k <<= 1) {
+        KJ_ROLLED
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            KJ_ROLLED
+            for (uint32_t t = (uint32_t)cx.w.lane; t < np / 2; t += 32) {
+                uint32_t i, p;
+                if (j == k >> 1) { const uint32_t b = t / j, o = t - b * j; i = b * k + o; p = b * k + k - 1u - o; }     // first step of a merge: mirrored pairs
+                else { const uint32_t b = t / j, o = t - b * j; i = b * 2u * j + o; p = i + j; }
+                if (p < n) {
+                    const uint64_t ki = q.key[i], kp = q.key[p];
+                    if (ki < kp) { q.key[i] = kp; q.key[p] = ki; const uint64_t x = q.pay[i]; q.pay[i] = q.pay[p]; q.pay[p] = x; }
+                }
+            }
+            cx.w.sync();
+        }
+    }
+    q.nsorted = n; q.next = 0; q.dirty = false;
+}
+// the top entry of a long read's queue: the head of the sorted run or the largest late entry.  Returns its key (0: empty) and slot (uniform).
+// min_val only grows over a read (MEM's longest, Greedy's best score): late entries below it can never be popped, and the scan drops them.
+static KJ_DEV uint64_t kj_queue_top_long(KjWarpCtx& cx, KjQueue<true>& q, uint32_t& slot, uint32_t min_val) {
+#if defined(KJ_EMU)
+    if (cx.w.lane == 0) { kj_emu_stats.lq_tops++; kj_emu_stats.lq_slots += 1u + (q.n - q.nsorted); }
+#endif
+    const uint64_t ks = q.next < q.nsorted ? q.key[q.next] : 0ull;
+    slot = q.next;
+    if (q.n == q.nsorted) return ks;
+    cx.w.sync();
+    uint64_t best = 0; uint32_t bs = 0, out = q.nsorted;
+    KJ_ROLLED
+    for (uint32_t b = q.nsorted; b < q.n; b += 32) {
+        const uint32_t s = b + (uint32_t)cx.w.lane; uint64_t k = 0, p = 0;
+        if (s < q.n) { k = q.key[s]; p = q.pay[s]; }
+        const bool live = s < q.n && kj_qval<true>(k) >= min_val; const uint32_t m = cx.w.ballot(live);
+        cx.w.sync();
+        if (live) { const uint32_t d = out + (uint32_t)kj_popc(m & lanemask_lt(cx.w.lane)); q.key[d] = k; q.pay[d] = p; if (k > best) { best = k; bs = d; } }
+        out += (uint32_t)kj_popc(m);
+    }
+    q.n = out;
+    cx.w.sync();
+    const uint64_t g = warp_max_u64(cx.w, best);
+    if (g <= ks) return ks;
+    slot = cx.w.shfl(bs, kj_ffs(cx.w.ballot(best == g)) - 1);
+    return g;
+}
+// remove the entry kj_queue_top_long returned and return its payload
+static KJ_DEV uint64_t kj_queue_take_long(KjWarpCtx& cx, KjQueue<true>& q, uint32_t slot) {
+    const uint64_t p = q.pay[slot];
+    if (slot < q.nsorted) { q.next++; return p; }
+    cx.w.sync();
+    if (cx.w.lane == 0) { q.key[slot] = q.key[q.n - 1]; q.pay[slot] = q.pay[q.n - 1]; }      // the late entries stay packed: a scan reads live ones only
+    q.n--;
+    cx.w.sync();
+    return p;
 }
 // After translation the fragments are ranked once (keys are unique): ord[k] = slot of the k-th entry in pop order.  As long as
 // no SEG piece has been pushed (rare) a pop is three broadcast shared-memory reads instead of a warp arg-max.
-static KJ_DEV void kj_queue_sort(KjWarpCtx& cx, KjQueue& q) {
+static KJ_DEV void kj_queue_sort(KjWarpCtx& cx, KjQueue<>& q) {
     cx.w.sync();
     KJ_ROLLED
     for (uint32_t i = (uint32_t)cx.w.lane; i < q.n; i += 32) {
@@ -365,7 +461,16 @@ static KJ_DEV void kj_queue_sort(KjWarpCtx& cx, KjQueue& q) {
     cx.w.sync();
 }
 // pop the top entry if its sort value is >= min_val (getNextFragment's gate, ConsumerThread.cpp:276-283)
-static KJ_DEV bool kj_queue_pop(KjWarpCtx& cx, KjQueue& q, uint32_t min_val, uint32_t& val, uint32_t& pay) {
+template <bool LONG = false>
+static KJ_DEV bool kj_queue_pop(KjWarpCtx& cx, KjQueue<LONG>& q, uint32_t min_val, uint32_t& val, typename KjW<LONG>::pay& pay) {
+    if constexpr (LONG) {
+        uint32_t slot; const uint64_t g = kj_queue_top_long(cx, q, slot, min_val);
+        if (g == 0) return false;
+        val = kj_qval<true>(g);
+        if (val < min_val) return false;
+        pay = kj_queue_take_long(cx, q, slot);
+        return true;
+    }
     if (!q.dirty) {
         if (q.next >= q.nsorted) return false;
         const uint32_t slot = q.ord[q.next]; const uint64_t k = q.key[slot];
@@ -391,7 +496,7 @@ static KJ_DEV bool kj_queue_pop(KjWarpCtx& cx, KjQueue& q, uint32_t min_val, uin
     return true;
 }
 // switch to scanning pops (a SEG piece is about to be pushed): consumed entries of the sorted prefix are cleared first
-static KJ_DEV void kj_queue_make_dirty(KjWarpCtx& cx, KjQueue& q) {
+static KJ_DEV void kj_queue_make_dirty(KjWarpCtx& cx, KjQueue<>& q) {
     if (q.dirty) return;
     cx.w.sync();
     KJ_ROLLED
@@ -411,7 +516,8 @@ static KJ_DEV uint32_t kj_nuc(uint8_t ch) {          // nuc2int (ConsumerThread.
 }
 // fragments = maximal stop-free runs of every frame (a stride-3 walk of an array); na1/na2 = array lengths of the two mates
 // (0 = mate absent), nframes = 3 for translated DNA, 1 for protein input (one "frame" whose residues sit at indices 3e).
-static KJ_DEV void kj_split_frames(KjWarpCtx& cx, KjQueue& q, const int na1, const int na2, const int n1, const int n2, const bool greedy, const int nframes) {
+template <bool LONG = false>
+static KJ_DEV void kj_split_frames(KjWarpCtx& cx, KjQueue<LONG>& q, const int na1, const int na2, const int n1, const int n2, const bool greedy, const int nframes) {
     const Warp& w = cx.w; const KjTables& tb = *cx.tb;
     const uint8_t* aa = cx.smem + cx.L.aa_off; const uint32_t st = cx.L.aa_stride;
     // fragments = maximal stop-free runs of every frame (a stride-3 walk of an array).  Per frame the stop positions
@@ -466,9 +572,11 @@ static KJ_DEV void kj_split_frames(KjWarpCtx& cx, KjQueue& q, const int na1, con
                     }
                     const bool leftover = e + 1 >= ne;
                     const int frame = (a & 1) ? (((n - 3 - r) % 3) + 3) % 3 : r;
-                    const uint32_t order = ((uint32_t)a << 16) | (leftover ? 40000u + (uint32_t)frame : (uint32_t)(r + 3 * (e + 1)));
+                    uint32_t order;
+                    if constexpr (LONG) order = kj_frag_order_long((uint32_t)a, leftover, (uint32_t)frame, (uint32_t)(r + 3 * (e + 1)));
+                    else order = ((uint32_t)a << 16) | (leftover ? 40000u + (uint32_t)frame : (uint32_t)(r + 3 * (e + 1)));
                     const bool emit = is_end && run_len >= m && (!greedy || run_score >= cx.rp->min_score);
-                    kj_queue_emit(cx, q, emit, greedy ? run_score : run_len, order, kj_qpay((uint32_t)a, false, run_start, run_len));
+                    kj_queue_emit<LONG>(cx, q, emit, greedy ? run_score : run_len, order, kj_qpay<LONG>((uint32_t)a, false, run_start, run_len));
                     if (sm[a]) { const int last = 31 - kj_clz(sm[a]); run_open[a] = e0 + last + 1; if (greedy) p_open[a] = w.shfl(pre[a], last); }
                     if (greedy) p_carry[a] = w.shfl(pre[a], 31);
                 }
@@ -480,7 +588,8 @@ static KJ_DEV void kj_split_frames(KjWarpCtx& cx, KjQueue& q, const int na1, con
 // The same splitting with the four arrays one after the other (one copy of the run logic instead of four interleaved ones: a quarter of the code).
 // Greedy only: there the instruction cache, not the dependent latency of this step, is the scarce resource (see kj_warp.h).  The
 // queue slots are filled in another order; the keys (value, reference insertion order) are the same, and only they decide the pop order.
-static KJ_DEV void kj_split_frames_rolled(KjWarpCtx& cx, KjQueue& q, const int na1, const int na2, const int n1, const int n2, const bool greedy, const int nframes) {
+template <bool LONG = false>
+static KJ_DEV void kj_split_frames_rolled(KjWarpCtx& cx, KjQueue<LONG>& q, const int na1, const int na2, const int n1, const int n2, const bool greedy, const int nframes) {
     const Warp& w = cx.w; const KjTables& tb = *cx.tb;
     const uint8_t* aa = cx.smem + cx.L.aa_off; const uint32_t st = cx.L.aa_stride;
     const uint32_t m = cx.rp->m;
@@ -516,9 +625,11 @@ static KJ_DEV void kj_split_frames_rolled(KjWarpCtx& cx, KjQueue& q, const int n
                 run_score = pre - p_before;
             }
             const bool leftover = e + 1 >= ne;
-            const uint32_t order = ((uint32_t)a << 16) | (leftover ? 40000u + (uint32_t)frame : (uint32_t)(r + 3 * (e + 1)));
+            uint32_t order;
+            if constexpr (LONG) order = kj_frag_order_long((uint32_t)a, leftover, (uint32_t)frame, (uint32_t)(r + 3 * (e + 1)));
+            else order = ((uint32_t)a << 16) | (leftover ? 40000u + (uint32_t)frame : (uint32_t)(r + 3 * (e + 1)));
             const bool emit = is_end && run_len >= m && (!greedy || run_score >= cx.rp->min_score);
-            kj_queue_emit(cx, q, emit, greedy ? run_score : run_len, order, kj_qpay((uint32_t)a, false, run_start, run_len));
+            kj_queue_emit<LONG>(cx, q, emit, greedy ? run_score : run_len, order, kj_qpay<LONG>((uint32_t)a, false, run_start, run_len));
             if (sm) { const int last = 31 - kj_clz(sm); run_open = e0 + last + 1; if (greedy) p_open = w.shfl(pre, last); }
             if (greedy) p_carry = w.shfl(pre, 31);
         }
@@ -527,7 +638,8 @@ static KJ_DEV void kj_split_frames_rolled(KjWarpCtx& cx, KjQueue& q, const int n
 
 // Both mates are translated and split in the SAME loops (array a = 2*mate + strand): the four arrays are independent, so
 // their load/ballot/bit-twiddling chains overlap instead of running back to back (the kernel is bound by dependent latency).
-static KJ_DEV void kj_translate_pair(KjWarpCtx& cx, KjQueue& q, const uint8_t* s1, int n1, bool do1, const uint8_t* s2, int n2, bool do2, bool greedy, const bool small_code) {
+template <bool LONG = false>
+static KJ_DEV void kj_translate_pair(KjWarpCtx& cx, KjQueue<LONG>& q, const uint8_t* s1, int n1, bool do1, const uint8_t* s2, int n2, bool do2, bool greedy, const bool small_code) {
     const Warp& w = cx.w; const KjTables& tb = *cx.tb;
     uint8_t* aa = cx.smem + cx.L.aa_off; const uint32_t st = cx.L.aa_stride;
     const int na1 = do1 ? n1 - 2 : 0, na2 = do2 ? n2 - 2 : 0;
@@ -552,8 +664,8 @@ static KJ_DEV void kj_translate_pair(KjWarpCtx& cx, KjQueue& q, const uint8_t* s
         }
     }
     w.sync();
-    if (small_code) kj_split_frames_rolled(cx, q, na1, na2, n1, n2, greedy, 3);      // Greedy is faster with the quarter-size splitting code (A/B)
-    else kj_split_frames(cx, q, na1, na2, n1, n2, greedy, 3);
+    if (small_code) kj_split_frames_rolled<LONG>(cx, q, na1, na2, n1, n2, greedy, 3);      // Greedy is faster with the quarter-size splitting code (A/B)
+    else kj_split_frames<LONG>(cx, q, na1, na2, n1, n2, greedy, 3);
 }
 
 // copy the characters of item (arr,start,len) into the contiguous fragment buffer
@@ -618,8 +730,11 @@ static KJ_DEV bool kj_seg_flags(KjWarpCtx& cx, int n, const bool compact) {
 // of its run of equal counts.  s_GetProb then walks the 20 sorted counts in the reference's order.
 // (a real function, like kj_seg_trim: the trim search is large and rarely the warp's hot path -- inlined copies of it cost
 // instruction-cache space in every kernel.  Returns best_start << 16 | best_end inside s[0..n2).)
-KJ_NOINLINE uint32_t kj_seg_trim_long(const Warp w, uint8_t* scratch, const uint8_t* s, int n2, const double* lnf) {
-    uint16_t* sv = (uint16_t*)scratch;                                // [20][32] counts, descending per lane
+// CntT: the count type (uint16_t; the long kernels' regions can exceed 65,535 residues: uint32_t, 3,840 of the scratch's >= 4,800 bytes);
+// RetT, SH: the packing of the result (start << SH | end).
+template <class CntT, class RetT, int SH>
+static KJ_DEV RetT kj_seg_trim_long_t(const Warp w, uint8_t* scratch, const uint8_t* s, int n2, const double* lnf) {
+    CntT* sv = (CntT*)scratch;                                        // [20][32] counts, descending per lane
     uint8_t* at = (uint8_t*)(sv + 20 * 32);                            // [20][32] letter stored at sorted position k
     uint8_t* where = at + 20 * 32;                                     // [20][32] sorted position of letter a
     int minlen = 1; if (n2 - KJ_SEG_MAXTRIM > minlen) minlen = n2 - KJ_SEG_MAXTRIM;
@@ -637,9 +752,9 @@ KJ_NOINLINE uint32_t kj_seg_trim_long(const Warp w, uint8_t* scratch, const uint
             #define KJ_SV_SWAP(p_, q_) { const uint32_t la_ = at[(p_) * 32 + ln], lb_ = at[(q_) * 32 + ln]; at[(p_) * 32 + ln] = (uint8_t)lb_; at[(q_) * 32 + ln] = (uint8_t)la_; \
                 where[la_ * 32 + ln] = (uint8_t)(q_); where[lb_ * 32 + ln] = (uint8_t)(p_); }
             #define KJ_SV_ADD(letter) { const uint32_t a_ = (letter) - 1u; uint32_t p_ = where[a_ * 32 + ln]; const uint32_t v_ = sv[p_ * 32 + ln]; uint32_t q_ = p_; \
-                while (q_ > 0 && sv[(q_ - 1) * 32 + ln] == v_) q_--; if (q_ != p_) KJ_SV_SWAP(p_, q_); sv[q_ * 32 + ln] = (uint16_t)(v_ + 1u); }
+                while (q_ > 0 && sv[(q_ - 1) * 32 + ln] == v_) q_--; if (q_ != p_) KJ_SV_SWAP(p_, q_); sv[q_ * 32 + ln] = (CntT)(v_ + 1u); }
             #define KJ_SV_DEL(letter) { const uint32_t a_ = (letter) - 1u; uint32_t p_ = where[a_ * 32 + ln]; const uint32_t v_ = sv[p_ * 32 + ln]; uint32_t q_ = p_; \
-                while (q_ < 19 && sv[(q_ + 1) * 32 + ln] == v_) q_++; if (q_ != p_) KJ_SV_SWAP(p_, q_); sv[q_ * 32 + ln] = (uint16_t)(v_ - 1u); }
+                while (q_ < 19 && sv[(q_ + 1) * 32 + ln] == v_) q_++; if (q_ != p_) KJ_SV_SWAP(p_, q_); sv[q_ * 32 + ln] = (CntT)(v_ - 1u); }
             KJ_ROLLED
             for (int t = 0; t < len; t++) KJ_SV_ADD(s[t]);
             KJ_ROLLED
@@ -672,7 +787,10 @@ KJ_NOINLINE uint32_t kj_seg_trim_long(const Warp w, uint8_t* scratch, const uint
             g_prob = mn; g_lend = wi; g_rend = wlen + wi - 1;
         }
     }
-    return ((uint32_t)g_lend << 16) | (uint32_t)g_rend;
+    return ((RetT)g_lend << SH) | (RetT)g_rend;
+}
+KJ_NOINLINE uint32_t kj_seg_trim_long(const Warp w, uint8_t* scratch, const uint8_t* s, int n2, const double* lnf) {
+    return kj_seg_trim_long_t<uint16_t, uint32_t, 16>(w, scratch, s, n2, lnf);
 }
 
 // s_Trim (blast_seg.c:1971-2015): the sub-window of s[0..n2) with minimal s_GetProb; first in
@@ -743,6 +861,12 @@ KJ_NOINLINE uint32_t kj_seg_trim(const Warp w, uint8_t* scratch, const uint8_t* 
     }
     return ((uint32_t)g_lend << 16) | (uint32_t)g_rend;
 }
+// the same for the long kernels: best_start << 32 | best_end
+KJ_NOINLINE uint64_t kj_seg_trim_wide(const Warp w, uint8_t* scratch, const uint8_t* s, int n2, const double* lnf) {
+    if (n2 > 127) return kj_seg_trim_long_t<uint32_t, uint64_t, 32>(w, scratch, s, n2, lnf);
+    const uint32_t t = kj_seg_trim(w, scratch, s, n2, lnf);
+    return ((uint64_t)(t >> 16) << 32) | (t & 0xffffu);
+}
 
 // s_SegSeq (blast_seg.c:2027-2113) on frag[s0 .. s0+n).  LEVEL 0 collects regions; LEVEL 1 is the
 // "trigger window fell into the left trim" recursion, of which the caller keeps only the last region
@@ -750,7 +874,7 @@ KJ_NOINLINE uint32_t kj_seg_trim(const Warp w, uint8_t* scratch, const uint8_t* 
 // Everything behind the window flags runs out of line (kj_seg_regions): a fragment with a low-complexity window is the exception, and
 // inlined copies of the region search cost instruction-cache space in the hot loop of every kernel.
 struct KjSegArgs { Warp w; const uint8_t* frag; const uint8_t* hf; KjSeg* segs; uint8_t* scratch; const double* lnf; int cap; uint32_t* err; };
-template <int LEVEL>
+template <int LEVEL, bool LONG>
 static KJ_DEV int kj_seg_level(const KjSegArgs& A, int s0, int n, KjSeg* segs, int nsegs) {
     const uint8_t* frag = A.frag; const uint8_t* hf = A.hf;
     if (KJ_SEG_WINDOW > n) return nsegs;
@@ -767,12 +891,16 @@ static KJ_DEV int kj_seg_level(const KjSegArgs& A, int s0, int n, KjSeg* segs, i
             while (j <= last && (hf[s0 + j - KJ_SEG_DOWNSET] & 2)) j++;
             const int hii = j - 1;               // s_FindHigh
             int leftend = loi - KJ_SEG_DOWNSET, rightend = hii + KJ_SEG_UPSET - 1;
+            if constexpr (LONG) {
+                const int n2 = rightend - leftend + 1; const uint64_t tr = kj_seg_trim_wide(A.w, A.scratch, frag + s0 + leftend, n2, A.lnf);
+                leftend += (int)(tr >> 32); rightend -= n2 - (int)(uint32_t)tr - 1;
+            } else
             { const int n2 = rightend - leftend + 1; const uint32_t tr = kj_seg_trim(A.w, A.scratch, frag + s0 + leftend, n2, A.lnf);
               leftend += (int)(tr >> 16); rightend -= n2 - (int)(tr & 0xffffu) - 1; }
             if (LEVEL == 0 && i + KJ_SEG_UPSET - 1 < leftend) {
                 const int lend = loi - KJ_SEG_DOWNSET, rend = leftend - 1;
                 KjSeg tmp; tmp.begin = -1; tmp.end = -1;
-                int got = kj_seg_level<1>(A, s0 + lend, rend - lend + 1, &tmp, 0);
+                int got = kj_seg_level<1, LONG>(A, s0 + lend, rend - lend + 1, &tmp, 0);
                 if (got > 0 && nsegs + 2 < A.cap) { if (A.w.lane == 0) segs[nsegs] = tmp; nsegs++; }
             }
             if (LEVEL == 0) {
@@ -793,9 +921,10 @@ static KJ_DEV int kj_seg_level(const KjSegArgs& A, int s0, int n, KjSeg* segs, i
     return nsegs;
 }
 // regions + s_MergeSegs (2122-2152) for a fragment whose window flags are set; returns the number of regions (ascending)
-KJ_NOINLINE int kj_seg_regions(const KjSegArgs A, int n) {
+template <bool LONG>
+static KJ_DEV int kj_seg_regions_t(const KjSegArgs& A, int n) {
     KjSeg* segs = A.segs;
-    int ns = kj_seg_level<0>(A, 0, n, segs, 0);
+    int ns = kj_seg_level<0, LONG>(A, 0, n, segs, 0);
     A.w.sync();
     if (ns > 1) {
         // creation order == ascending; the reference walks the reversed list from its head
@@ -821,13 +950,17 @@ KJ_NOINLINE int kj_seg_regions(const KjSegArgs A, int n) {
     }
     return ns;
 }
+KJ_NOINLINE int kj_seg_regions(const KjSegArgs A, int n) { return kj_seg_regions_t<false>(A, n); }
+KJ_NOINLINE int kj_seg_regions_long(const KjSegArgs A, int n) { return kj_seg_regions_t<true>(A, n); }
 // full SEG on frag[0..n): flags (inline, every fragment), regions (out of line, rare)
+template <bool LONG = false>
 static KJ_DEV int kj_seg(KjWarpCtx& cx, int n, const bool compact) {
     if (n < KJ_SEG_WINDOW) return 0;
     if (!kj_seg_flags(cx, n, compact)) return 0;                      // no window at or below locut: s_SegSeq cannot trigger
     KjSegArgs A; A.w = cx.w; A.frag = cx.smem + cx.L.frag_off; A.hf = cx.smem + cx.L.hflag_off; A.segs = (KjSeg*)(cx.smem + cx.L.segs_off);
     A.scratch = cx.smem + cx.L.segcnt_off; A.lnf = cx.ix->lnfact; A.cap = (int)KJ_SEG_CAP(cx.rp->max_frag); A.err = cx.err;
-    return kj_seg_regions(A, n);
+    if constexpr (LONG) return kj_seg_regions_long(A, n);
+    else return kj_seg_regions(A, n);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -948,10 +1081,11 @@ static KJ_DEV uint32_t kj_ids_and_lca(KjWarpCtx& cx, uint32_t nkept) {
 // ---------------------------------------------------------------------------------------------
 
 // SEG gate of getNextFragment (ConsumerThread.cpp:285-339): returns true if the item was split (pieces pushed)
-static KJ_DEV bool kj_seg_gate(KjWarpCtx& cx, KjQueue& q, uint32_t arr, uint32_t start, uint32_t len, bool greedy) {
-    int ns = kj_seg(cx, (int)len, greedy);
+template <bool LONG = false>
+static KJ_DEV bool kj_seg_gate(KjWarpCtx& cx, KjQueue<LONG>& q, uint32_t arr, uint32_t start, uint32_t len, bool greedy) {
+    int ns = kj_seg<LONG>(cx, (int)len, greedy);
     if (ns == 0) return false;
-    kj_queue_make_dirty(cx, q);
+    if constexpr (!LONG) kj_queue_make_dirty(cx, q);          // (the long kernels' queue keeps late entries apart: kj_queue_top_long)
     const KjSeg* segs = (const KjSeg*)(cx.smem + cx.L.segs_off);
     const uint8_t* frag = cx.smem + cx.L.frag_off; const KjTables& tb = *cx.tb;
     uint32_t st = 0;
@@ -961,7 +1095,7 @@ static KJ_DEV bool kj_seg_gate(KjWarpCtx& cx, KjQueue& q, uint32_t arr, uint32_t
         if (plen > (int)cx.rp->m) {                                        // strict '>' for pieces (298, 312)
             uint32_t val = (uint32_t)plen; bool ok = true;
             if (greedy) { uint32_t sc = 0; for (int t = 0; t < plen; t++) { uint32_t a = frag[st + t]; sc += (uint32_t)tb.b62[a][a]; } val = sc; ok = sc >= cx.rp->min_score; }
-            kj_queue_emit(cx, q, cx.w.lane == 0 && ok, val, KJ_ORDER_LATE + q.late, kj_qpay(arr, true, start + 3u * st, (uint32_t)plen));
+            kj_queue_emit<LONG>(cx, q, cx.w.lane == 0 && ok, val, (LONG ? KJ_ORDER_LATE_LONG : KJ_ORDER_LATE) + q.late, kj_qpay<LONG>(arr, true, start + 3u * st, (uint32_t)plen));
             if (ok) q.late++;
         }
         if (s < ns) st = (uint32_t)segs[s].end + 1u;
@@ -970,11 +1104,13 @@ static KJ_DEV bool kj_seg_gate(KjWarpCtx& cx, KjQueue& q, uint32_t arr, uint32_t
 }
 
 // One popped fragment: search, deferred SEG gate, merge into the kept list.  Returns true if it had a match >= L.
-template <class IdxT>
-static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t& longest, uint32_t& nkept) {
+template <class IdxT, bool LONG = false>
+static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue<LONG>& q, typename KjW<LONG>::pay pay, uint32_t& longest, uint32_t& nkept) {
     const Warp& w = cx.w; const KjDevIndex& ix = *cx.ix; const KjRunParams& rp = *cx.rp;
     const uint8_t* frag = cx.smem + cx.L.frag_off;
-    const uint32_t arr = pay >> 30, start = (pay >> 14) & 0x7fffu, len = pay & 0x3fffu; const bool segchecked = (pay >> 29) & 1u;
+    uint32_t arr, start, len; bool segchecked;
+    if constexpr (LONG) kj_qpay_dec<LONG>(pay, arr, segchecked, start, len);
+    else { arr = pay >> 30; start = (pay >> 14) & 0x7fffu; len = pay & 0x3fffu; segchecked = (pay >> 29) & 1u; }
         kj_load_frag(cx, arr, start, len);
         // SEG is deferred until the fragment is known to matter: every match inside a SEG piece is also a match inside the
         // whole fragment (for each end position the piece's match is a suffix of the fragment's), so a fragment whose
@@ -1048,7 +1184,9 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
                 if (lmax > item_best) { item_best = lmax; item_cnt = 0; }
                 L = lmax;
                 const uint32_t wm = w.ballot(l == item_best && l > 0);
-                if (l == item_best && l > 0) { KjKept* k = kj_kept_ptr(cx, nkept + item_cnt + (uint32_t)kj_popc(wm & lanemask_lt(w.lane))); k->lo = (uint64_t)cur.lo; k->len = (uint32_t)(cur.hi - cur.lo); k->aux = (arr << 29) | ((start + 3u * (uint32_t)cur.i) << 14) | l; }      // aux: where the matched text lies (verbose output)
+                // aux: where the matched text lies (verbose output).  The long kernels keep its 21-bit position only: every kept match is `longest` long.
+                if (l == item_best && l > 0) { KjKept* k = kj_kept_ptr(cx, nkept + item_cnt + (uint32_t)kj_popc(wm & lanemask_lt(w.lane))); k->lo = (uint64_t)cur.lo; k->len = (uint32_t)(cur.hi - cur.lo);
+                                               k->aux = LONG ? (arr << 29) | (start + 3u * (uint32_t)cur.i) : (arr << 29) | ((start + 3u * (uint32_t)cur.i) << 14) | l; }
                 item_cnt += (uint32_t)kj_popc(wm);
             }
             jhi -= 32;
@@ -1059,7 +1197,7 @@ static KJ_DEV bool kj_mem_item(KjWarpCtx& cx, KjQueue& q, uint32_t pay, uint32_t
         w.sync();
         // the SEG gate of getNextFragment (ConsumerThread.cpp:285-339), now that the fragment has a match >= L: if SEG masks
         // something the fragment is replaced by its pieces exactly as in the reference and this search result is dropped
-        if (item_cnt > 0 && rp.seg && !segchecked && kj_seg_gate(cx, q, arr, start, len, false)) return true;
+        if (item_cnt > 0 && rp.seg && !segchecked && kj_seg_gate<LONG>(cx, q, arr, start, len, false)) return true;
         if (item_cnt > 0) {
             // winners were appended j-descending; the reference's chain (greedyExact, bwt.c:347-380) is newest (smallest j) first.  The
             // kaijux / kaijup front-ends search with maxMatches(..., 1) instead, whose list keeps the first-found match at the head and
@@ -1098,30 +1236,31 @@ KJ_NOINLINE uint32_t kj_emit_text(const Warp w, char* text, uint32_t at, uint32_
     if (w.lane == 0) text[at + len] = ',';
     return at + len + 1u;
 }
-static KJ_DEV void kj_emit_fragments_mem(KjWarpCtx& cx, uint32_t nkept) {
+template <bool LONG = false>
+static KJ_DEV void kj_emit_fragments_mem(KjWarpCtx& cx, uint32_t nkept, uint32_t longest) {
     KJ_ROLLED
     for (uint32_t e = 0; e < nkept; e++) {
         const uint32_t aux = kj_kept_ptr(cx, e)->aux;
         if (!(aux >> 31)) continue;
-        const uint32_t arr = (aux >> 29) & 3u, pos = (aux >> 14) & 0x7fffu, len = aux & 0x3fffu;
+        const uint32_t arr = (aux >> 29) & 3u, pos = LONG ? aux & 0x1fffffffu : (aux >> 14) & 0x7fffu, len = LONG ? longest : aux & 0x3fffu;
         const uint32_t at = kj_emit_text(cx.w, cx.text, cx.text_len, cx.text_cap, cx.smem + cx.L.aa_off + arr * cx.L.aa_stride + pos, 3u, len, cx.tb->letters);
         if (at == 0xffffffffu) { if (cx.w.lane == 0) kj_flag_error(cx, 128u); return; }
         cx.text_len = at;
     }
     cx.w.sync();
 }
-template <class IdxT>
-static KJ_DEV uint32_t kj_classify_mem(KjWarpCtx& cx, KjQueue& q, uint32_t& best_out) {
+template <class IdxT, bool LONG = false>
+static KJ_DEV uint32_t kj_classify_mem(KjWarpCtx& cx, KjQueue<LONG>& q, uint32_t& best_out) {
     uint32_t longest = 0, nkept = 0;                                      // uniform
-    uint32_t val, pay;
+    uint32_t val; typename KjW<LONG>::pay pay;
     KJ_ROLLED
-    while (kj_queue_pop(cx, q, longest, val, pay)) kj_mem_item<IdxT>(cx, q, pay, longest, nkept);
+    while (kj_queue_pop<LONG>(cx, q, longest, val, pay)) kj_mem_item<IdxT, LONG>(cx, q, pay, longest, nkept);
     best_out = 0;
     if (nkept == 0) return KJ_TAX_BAD;
     cx.w.sync();
     uint32_t t = kj_ids_and_lca<IdxT>(cx, nkept);
     if (t != KJ_TAX_BAD) best_out = longest;
-    if (cx.text && t != KJ_TAX_BAD) kj_emit_fragments_mem(cx, nkept);
+    if (cx.text && t != KJ_TAX_BAD) kj_emit_fragments_mem<LONG>(cx, nkept, longest);
     return t;
 }
 
@@ -1129,13 +1268,14 @@ static KJ_DEV uint32_t kj_classify_mem(KjWarpCtx& cx, KjQueue& q, uint32_t& best
 // ConsumerThread::doWork for one item (ConsumerThread.cpp:630-749): gates, translation, mode dispatch.
 // Returns the compact taxon (KJ_TAX_BAD = unclassified).
 // ---------------------------------------------------------------------------------------------
-template <class IdxT> static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, int n1, int n2, uint32_t& best_out);
+template <class IdxT, bool LONG = false> static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue<LONG>& q, double query_len, uint32_t& best_out);
 
 // Protein input (-p, ConsumerThread.cpp:640-646, 659-696): the read is upper-cased and split at every letter outside
 // "ACDEFGHIKLMNPQRSTVWY"; pieces of at least m residues (Greedy: and score >= min_score) are queued in order, the tail last.
 // The residues are stored like one reading frame of a translated read (residue e at array index 3e), so the queue
 // payloads, kj_load_frag and the SEG pieces need no second addressing mode.
-static KJ_DEV void kj_protein_fragments(KjWarpCtx& cx, KjQueue& q, const uint8_t* s1, int n1, bool greedy, const bool small_code) {
+template <bool LONG = false>
+static KJ_DEV void kj_protein_fragments(KjWarpCtx& cx, KjQueue<LONG>& q, const uint8_t* s1, int n1, bool greedy, const bool small_code) {
     const Warp& w = cx.w; const KjTables& tb = *cx.tb;
     uint8_t* aa = cx.smem + cx.L.aa_off;
     KJ_ROLLED
@@ -1144,8 +1284,8 @@ static KJ_DEV void kj_protein_fragments(KjWarpCtx& cx, KjQueue& q, const uint8_t
         aa[3 * t] = (u >= 'A' && u <= 'Z') ? tb.aa_index[u - 'A'] : (uint8_t)0;
     }
     w.sync();
-    if (small_code) kj_split_frames_rolled(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
-    else kj_split_frames(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
+    if (small_code) kj_split_frames_rolled<LONG>(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
+    else kj_split_frames<LONG>(cx, q, 3 * n1 - 2, 0, n1, 0, greedy, 1);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1160,7 +1300,7 @@ static KJ_HD uint32_t kj_prep_pays_off(const KjRunParams& p) { return 16u + 8u *
 static KJ_HD uint32_t kj_prep_ords_off(const KjRunParams& p) { return kj_prep_pays_off(p) + 4u * kj_align(p.item_cap, 2); }
 static KJ_HD uint32_t kj_prep_aa_off(const KjRunParams& p) { return kj_align(kj_prep_ords_off(p) + kj_align(p.item_cap, 8), 16); }
 static KJ_HD uint32_t kj_prep_stride(const KjRunParams& p) { return kj_align(kj_prep_aa_off(p) + 4u * kj_align(p.max_len + 4, 8), 16); }
-static KJ_DEV void kj_prep_store(KjWarpCtx& cx, const KjQueue& q, bool ok, uint8_t* rec) {
+static KJ_DEV void kj_prep_store(KjWarpCtx& cx, const KjQueue<>& q, bool ok, uint8_t* rec) {
     const Warp& w = cx.w; const KjRunParams& rp = *cx.rp;
     w.sync();
     if (w.lane == 0) *(uint32_t*)rec = ok ? q.n : 0xffffffffu;
@@ -1174,7 +1314,7 @@ static KJ_DEV void kj_prep_store(KjWarpCtx& cx, const KjQueue& q, bool ok, uint8
     }
     w.sync();
 }
-static KJ_DEV bool kj_prep_load(KjWarpCtx& cx, KjQueue& q, const uint8_t* rec) {
+static KJ_DEV bool kj_prep_load(KjWarpCtx& cx, KjQueue<>& q, const uint8_t* rec) {
     const Warp& w = cx.w; const KjRunParams& rp = *cx.rp;
     const uint32_t n = *(const uint32_t*)rec;
     if (n == 0xffffffffu) return false;
@@ -1189,11 +1329,13 @@ static KJ_DEV bool kj_prep_load(KjWarpCtx& cx, KjQueue& q, const uint8_t* rec) {
     return true;
 }
 
-template <int MODE, class IdxT, int ROLE = 0>
+// LONG: the long-read instance (ROLE 0 only)
+template <int MODE, class IdxT, int ROLE = 0, bool LONG = false>
 static KJ_DEV uint32_t kj_classify_item(KjWarpCtx& cx, const uint8_t* s1, int n1, const uint8_t* s2, int n2, bool paired, uint32_t& best_out, uint8_t* rec = nullptr) {
+    static_assert(!LONG || ROLE == 0, "the long-read kernels run every item in one kernel");
     const KjRunParams& rp = *cx.rp;
     best_out = 0; cx.nids = 0;
-    KjQueue q; q.key = (uint64_t*)(cx.smem + cx.L.qkey_off); q.pay = (uint32_t*)(cx.smem + cx.L.qpay_off);
+    KjQueue<LONG> q; q.key = (uint64_t*)(cx.smem + cx.L.qkey_off); q.pay = (typename KjW<LONG>::pay*)(cx.smem + cx.L.qpay_off);
     q.ord = cx.smem + cx.L.qord_off; q.cap = rp.item_cap; q.n = 0; q.late = 0; q.next = 0; q.nsorted = 0; q.dirty = true;
     const bool greedy = MODE == 1;
     // the one-kernel Greedy path trades the interleaved (4 arrays at once) frame splitting for a quarter of its code; the front-end kernel of the
@@ -1204,19 +1346,23 @@ static KJ_DEV uint32_t kj_classify_item(KjWarpCtx& cx, const uint8_t* s1, int n1
         bool ok = true;
         if (rp.protein) {
             if (n1 < (int)rp.m) ok = false;                                  // (640-646)
-            else kj_protein_fragments(cx, q, s1, n1, greedy, small_code);
+            else kj_protein_fragments<LONG>(cx, q, s1, n1, greedy, small_code);
         } else {
             // short-read gate (648-653): SE len1 < 3m; PE only if BOTH mates are short
             if ((!paired && n1 < m3) || (paired && n1 < m3 && n2 < m3)) ok = false;
-            else kj_translate_pair(cx, q, s1, n1, n1 >= m3, s2, n2, paired && n2 >= m3, greedy, small_code);   // a short mate is skipped individually (699, 705)
+            else kj_translate_pair<LONG>(cx, q, s1, n1, n1 >= m3, s2, n2, paired && n2 >= m3, greedy, small_code);   // a short mate is skipped individually (699, 705)
         }
+        // a long read's queue holds tens of thousands of fragments: ranked once in both modes, so that no pop scans them all
+        if constexpr (LONG) { if (ok) kj_queue_rank_long(cx, q); }
+        else {
         if (ok && MODE == 1) kj_queue_sort(cx, q);     // greedy pops every fragment (and many variants): ranking once pays (A/B); MEM stops after a few pops (slower with it)
-        if (ROLE == 1) { kj_prep_store(cx, q, ok, rec); return KJ_TAX_BAD; }
+        if constexpr (ROLE == 1) { kj_prep_store(cx, q, ok, rec); return KJ_TAX_BAD; }
+        }
         if (!ok) return KJ_TAX_BAD;
-    } else if (!kj_prep_load(cx, q, rec)) return KJ_TAX_BAD;
+    } else if constexpr (!LONG) { if (!kj_prep_load(cx, q, rec)) return KJ_TAX_BAD; }
     double query_len;                                                    // E-value query length (659, 698, 704)
     if (rp.protein) query_len = (double)n1;
     else { query_len = (double)n1 / 3.0; if (paired) query_len += (double)n2 / 3.0; }
-    if (MODE == 0) return kj_classify_mem<IdxT>(cx, q, best_out);
-    else return kj_classify_greedy<IdxT>(cx, q, query_len, best_out);
+    if (MODE == 0) return kj_classify_mem<IdxT, LONG>(cx, q, best_out);
+    else return kj_classify_greedy<IdxT, LONG>(cx, q, query_len, best_out);
 }

@@ -10,31 +10,37 @@
 #pragma once
 #include "kj_core.h"
 
+template <bool LONG = false>
 struct alignas(16) KjVariant {
     uint64_t lo, hi;           // resume interval (Fragment::si0/si1, ConsumerThread.hpp:52)
-    uint32_t pay;              // source run: arr(2) start(15) len(14) -- len already truncated
+    typename KjW<LONG>::pay pay;   // source run (a queue payload, kj_qpay) -- len already truncated
     int32_t diff;              // accumulated substitution score delta (Fragment::diff)
-    uint16_t matchlen; uint8_t num_mm; uint8_t pad;
+    typename KjW<LONG>::pos matchlen; uint8_t num_mm; uint8_t pad;
     uint32_t subs[KJ_MAX_MM];  // pos << 5 | letter
     uint32_t pad2;
 };
-static_assert(sizeof(KjVariant) == 64, "KjVariant is one 64-byte record");
+static_assert(sizeof(KjVariant<>) == 64, "KjVariant is one 64-byte record");
 // per-warp ring in global scratch: keys[variant_cap] (scanned, contiguous) followed by the payload records
-static KJ_HD uint32_t kj_greedy_scratch_bytes(const KjRunParams& rp) { return rp.mode == 1 ? rp.variant_cap * (uint32_t)(sizeof(KjVariant) + 8u) : 64u; }
+template <bool LONG = false>
+static KJ_HD uint32_t kj_greedy_scratch_bytes(const KjRunParams& rp) { return rp.mode == 1 ? rp.variant_cap * (uint32_t)(sizeof(KjVariant<LONG>) + 8u) : 64u; }
 
-struct KjMatch { uint64_t lo; uint32_t len; uint16_t qi, ql; };    // one SI: interval + query position/length
+template <bool LONG = false>
+struct KjMatch { uint64_t lo; uint32_t len; typename KjW<LONG>::pos qi, ql; };    // one SI: interval + query position/length
+static_assert(sizeof(KjMatch<false>) == 16 && sizeof(KjMatch<true>) == 24, "kj_smem_layout sizes the result arrays with these");
 
 // key(s) = kj_qkey(score, order), 0 = free.  (Keeping the first keys in shared memory was slower in an A/B run.)
-struct KjVQueue { uint64_t* gkey; KjVariant* v; uint32_t n, live;      // n: high-water mark, live: entries not yet popped (uniform)
+template <bool LONG = false>
+struct KjVQueue { uint64_t* gkey; KjVariant<LONG>* v; uint32_t n, live;      // n: high-water mark, live: entries not yet popped (uniform)
     KJ_DEV uint64_t& key(uint32_t s) const { return gkey[s]; } };
 
 // compact live variants to the front (called when the ring is full); out of line: rare.  Returns the number of live entries.
-KJ_NOINLINE uint32_t kj_vq_compact_fn(const Warp w, uint64_t* gkey, KjVariant* v, uint32_t n) {
+template <class V>
+static KJ_DEV uint32_t kj_vq_compact_t(const Warp& w, uint64_t* gkey, V* v, uint32_t n) {
     uint32_t out = 0;
     KJ_ROLLED
     for (uint32_t b = 0; b < n; b += 32) {
         uint32_t s = b + (uint32_t)w.lane; bool live = s < n && gkey[s] != 0;
-        KjVariant tmp; uint64_t tk = 0; if (live) { tmp = v[s]; tk = gkey[s]; }
+        V tmp; uint64_t tk = 0; if (live) { tmp = v[s]; tk = gkey[s]; }
         uint32_t mask = w.ballot(live);
         w.sync();
         if (live) { const uint32_t d = out + (uint32_t)kj_popc(mask & lanemask_lt(w.lane)); v[d] = tmp; gkey[d] = tk; }
@@ -43,7 +49,14 @@ KJ_NOINLINE uint32_t kj_vq_compact_fn(const Warp w, uint64_t* gkey, KjVariant* v
     }
     return out;
 }
-static KJ_DEV void kj_vq_compact(KjWarpCtx& cx, KjVQueue& vq) { vq.n = kj_vq_compact_fn(cx.w, vq.gkey, vq.v, vq.n); vq.live = vq.n; }
+KJ_NOINLINE uint32_t kj_vq_compact_fn(const Warp w, uint64_t* gkey, KjVariant<>* v, uint32_t n) { return kj_vq_compact_t(w, gkey, v, n); }
+KJ_NOINLINE uint32_t kj_vq_compact_long_fn(const Warp w, uint64_t* gkey, KjVariant<true>* v, uint32_t n) { return kj_vq_compact_t(w, gkey, v, n); }
+template <bool LONG>
+static KJ_DEV void kj_vq_compact(KjWarpCtx& cx, KjVQueue<LONG>& vq) {
+    if constexpr (LONG) vq.n = kj_vq_compact_long_fn(cx.w, vq.gkey, vq.v, vq.n);
+    else vq.n = kj_vq_compact_fn(cx.w, vq.gkey, vq.v, vq.n);
+    vq.live = vq.n;
+}
 
 // inclusive warp scan helper (uint32)
 static KJ_DEV uint32_t kj_scan_incl(const Warp& w, uint32_t v) {
@@ -51,15 +64,18 @@ static KJ_DEV uint32_t kj_scan_incl(const Warp& w, uint32_t v) {
     return v;
 }
 
-template <class IdxT>
-static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double query_len, uint32_t& best_out) {
+// LONG: positions, lengths and prefix sums in 32 bits, scores unclamped, and the match start rides above bit KJ_LONG_LO_BITS of `lo` (not 48)
+template <class IdxT, bool LONG>
+static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue<LONG>& q, double query_len, uint32_t& best_out) {
+    typedef typename KjW<LONG>::pos PosT; typedef KjMatch<LONG> Match;
+    constexpr int QI_SHIFT = LONG ? KJ_LONG_LO_BITS : 48; constexpr uint64_t LO_MASK = (1ull << QI_SHIFT) - 1ull;
     const Warp& w = cx.w; const KjDevIndex& ix = *cx.ix; const KjRunParams& rp = *cx.rp; const KjTables& tb = *cx.tb;
     uint8_t* frag = cx.smem + cx.L.frag_off;
-    uint16_t* pre = (uint16_t*)(cx.smem + cx.L.pre_off);               // pre[t] = sum diag(frag[0..t))
-    KjMatch* res = (KjMatch*)(cx.smem + cx.L.res_off);                  // per-j chain results, then recorded matches
-    KjMatch* cls = (KjMatch*)(cx.smem + cx.L.res2_off);                 // recorded matches sorted into classes
+    PosT* pre = (PosT*)(cx.smem + cx.L.pre_off);                         // pre[t] = sum diag(frag[0..t))
+    Match* res = (Match*)(cx.smem + cx.L.res_off);                      // per-j chain results, then recorded matches
+    Match* cls = (Match*)(cx.smem + cx.L.res2_off);                     // recorded matches sorted into classes
     uint32_t* psub = (uint32_t*)(cx.smem + cx.L.ids_off + 64u);           // the id set is only filled after the loop
-    KjVQueue vq; vq.gkey = (uint64_t*)cx.gscratch; vq.v = (KjVariant*)((uint8_t*)cx.gscratch + 8u * rp.variant_cap); vq.n = 0; vq.live = 0;
+    KjVQueue<LONG> vq; vq.gkey = (uint64_t*)cx.gscratch; vq.v = (KjVariant<LONG>*)((uint8_t*)cx.gscratch + 8u * rp.variant_cap); vq.n = 0; vq.live = 0;
     uint32_t best = 0, nbest = 0;                                        // best_match_score, best_matches_SI.size()  (uniform)
     best_out = 0;
 
@@ -72,7 +88,8 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
         for (uint32_t s = (uint32_t)w.lane; s < vq.n; s += 32) { uint64_t k = vq.key(s); if (k > kb) { kb = k; slot_b = s; } }
         uint64_t gb = warp_max_u64(w, kb);
         uint64_t ka = 0, ga = 0; uint32_t slot_a = 0;
-        if (!q.dirty) { if (q.next < q.nsorted) { slot_a = q.ord[q.next]; ga = q.key[slot_a]; } }      // sorted prefix: the top is known
+        if constexpr (LONG) ga = kj_queue_top_long(cx, q, slot_a, best);
+        else if (!q.dirty) { if (q.next < q.nsorted) { slot_a = q.ord[q.next]; ga = q.key[slot_a]; } }      // sorted prefix: the top is known
         else {
             KJ_ROLLED
             for (uint32_t s = (uint32_t)w.lane; s < q.n; s += 32) { uint64_t k = q.key[s]; if (k > ka) { ka = k; slot_a = s; } }
@@ -80,17 +97,18 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
         }
         const uint64_t g = ga > gb ? ga : gb;
         if (g == 0) break;
-        if ((uint32_t)(g >> 32) < best) break;
+        if (kj_qval<LONG>(g) < best) break;
         uint32_t arr, start, len, num_mm = 0, matchlen = 0; int diff = 0; uint64_t si0 = 0, si1 = 0; bool segchecked; uint32_t nsub = 0; uint32_t mysub = 0;
         if (ga >= gb) {
-            uint32_t p = 0;
-            if (!q.dirty) { p = q.pay[slot_a]; q.next++; }
+            typename KjW<LONG>::pay p = 0;
+            if constexpr (LONG) p = kj_queue_take_long(cx, q, slot_a);
+            else if (!q.dirty) { p = q.pay[slot_a]; q.next++; }
             else {
                 int src = kj_ffs(w.ballot(ka == g)) - 1;
                 if (w.lane == src) { p = q.pay[slot_a]; q.key[slot_a] = 0; }
                 p = w.shfl(p, src);
             }
-            arr = p >> 30; segchecked = (p >> 29) & 1u; start = (p >> 14) & 0x7fffu; len = p & 0x3fffu;
+            kj_qpay_dec<LONG>(p, arr, segchecked, start, len);
 #if defined(KJ_EMU)
             if (w.lane == 0) kj_emu_stats.pops_frag++;
 #endif
@@ -99,8 +117,9 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             if (w.lane == 0) kj_emu_stats.pops_var++;
 #endif
             int src = kj_ffs(w.ballot(kb == g)) - 1; uint32_t sl = w.shfl(slot_b, src);
-            const KjVariant& V = vq.v[sl];
-            uint32_t p = V.pay; arr = p >> 30; start = (p >> 14) & 0x7fffu; len = p & 0x3fffu; segchecked = true;
+            const KjVariant<LONG>& V = vq.v[sl];
+            if constexpr (LONG) { kj_qpay_dec<LONG>(V.pay, arr, segchecked, start, len); segchecked = true; }
+            else { uint32_t p = V.pay; arr = p >> 30; start = (p >> 14) & 0x7fffu; len = p & 0x3fffu; segchecked = true; }
             num_mm = V.num_mm; matchlen = V.matchlen; diff = V.diff; si0 = V.lo; si1 = V.hi; nsub = num_mm;
             if ((uint32_t)w.lane < nsub) { mysub = V.subs[w.lane]; psub[w.lane] = mysub; }        // parent substitutions, re-read when variants are pushed
             w.sync();
@@ -110,7 +129,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
         kj_load_frag(cx, arr, start, len);
         if ((uint32_t)w.lane < nsub) frag[mysub >> 5] = (uint8_t)(mysub & 31u);
         w.sync();
-        if (rp.seg && !segchecked && kj_seg_gate(cx, q, arr, start, len, true)) continue;
+        if (rp.seg && !segchecked && kj_seg_gate<LONG>(cx, q, arr, start, len, true)) continue;
 
         // prefix sums of the BLOSUM62 diagonal (calcScore, ConsumerThread.cpp:397-421)
         {
@@ -120,7 +139,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                 uint32_t t = b + (uint32_t)w.lane; uint32_t a = t < len ? frag[t] : 0u;
                 uint32_t d = t < len ? (uint32_t)tb.b62[a][a] : 0u;
                 uint32_t sc = kj_scan_incl(w, d) + carry;
-                if (t < len) pre[t + 1] = (uint16_t)sc;
+                if (t < len) pre[t + 1] = (PosT)sc;
                 carry = w.shfl(sc, 31);
             }
             if (w.lane == 0) pre[0] = 0;
@@ -143,7 +162,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             const IdxT lo = one.lo, hi = one.hi; const int i = one.i;
             uint32_t l = len - (uint32_t)i;
             uint32_t Lreq = (num_mm == rp.e) ? rp.m : matchlen;           // ConsumerThread.cpp:445-450
-            if (l >= Lreq) { if (w.lane == 0) { cls[0].lo = (uint64_t)lo; cls[0].len = (uint32_t)(hi - lo); cls[0].qi = (uint16_t)i; cls[0].ql = (uint16_t)l; } nrec = 1; }
+            if (l >= Lreq) { if (w.lane == 0) { cls[0].lo = (uint64_t)lo; cls[0].len = (uint32_t)(hi - lo); cls[0].qi = (PosT)i; cls[0].ql = (PosT)l; } nrec = 1; }
             w.sync();
         } else {
             // maxMatches(f, seq, len, seed_length, 0) (bwt.c:261-296): one chain per end position j.  Every chain above the `i<=1` break
@@ -198,7 +217,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                 const bool valid = act && w.lane <= cut;
                 if (valid) {
                     if (cur.st == KJ_ST_OPEN) { res[j].lo = 0; res[j].len = 0; res[j].qi = 0; res[j].ql = 0; }       // skipped: provably not recorded
-                    else { res[j].lo = (uint64_t)cur.lo; res[j].len = (uint32_t)(cur.hi - cur.lo); res[j].qi = (uint16_t)cur.i; res[j].ql = (uint16_t)(j - cur.i + 1); }
+                    else { res[j].lo = (uint64_t)cur.lo; res[j].len = (uint32_t)(cur.hi - cur.lo); res[j].qi = (PosT)cur.i; res[j].ql = (PosT)(j - cur.i + 1); }
                 }
                 { const bool qual = valid && cur.st == KJ_ST_EXACT && j - cur.i + 1 >= L; const uint32_t mn = warp_min_u32(w, qual ? (uint32_t)cur.i : 0xffffffffu); if (mn < qi_above) qi_above = mn; }
                 const int nact = (jhi - (L - 1) + 1) < 32 ? (jhi - (L - 1) + 1) : 32;
@@ -222,7 +241,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                 int t = b + w.lane; int j = (int)len - 1 - t; bool rec = false;
                 {
                     uint32_t mine = 0xffffffffu;                           // my start if my chain qualifies
-                    if (t < nproc) { KjMatch r = res[j]; if (r.ql >= (uint32_t)L) mine = r.qi; }
+                    if (t < nproc) { Match r = res[j]; if (r.ql >= (uint32_t)L) mine = r.qi; }
                     uint32_t pm = mine;                                    // inclusive prefix minimum over the lanes
                     for (int dd = 1; dd < 32; dd <<= 1) { const uint32_t o = w.shfl(pm, w.lane - dd); if (w.lane >= dd && o < pm) pm = o; }
                     uint32_t ex = w.shfl(pm, w.lane - 1); if (w.lane == 0) ex = 0xffffffffu;     // exclusive
@@ -231,7 +250,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                     { const uint32_t last = w.shfl(pm, 31); if (last < cur_qi) cur_qi = last; }
                 }
                 uint32_t mk = w.ballot(rec);
-                if (rec) { KjMatch r = res[j]; cls[nrec + (uint32_t)kj_popc(mk & lanemask_lt(w.lane))] = r; }   // found order, temporarily in cls
+                if (rec) { Match r = res[j]; cls[nrec + (uint32_t)kj_popc(mk & lanemask_lt(w.lane))] = r; }   // found order, temporarily in cls
                 nrec += (uint32_t)kj_popc(mk);
             }
             w.sync();
@@ -240,7 +259,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             for (uint32_t b = 0; b < nrec; b += 32) {
                 uint32_t t = b + (uint32_t)w.lane;
                 if (t < nrec) {
-                    KjMatch r = cls[t]; uint32_t pos = 0;
+                    Match r = cls[t]; uint32_t pos = 0;
                     KJ_ROLLED
                     for (uint32_t u = 0; u < nrec; u++) { uint32_t q2 = cls[u].ql; pos += (q2 > r.ql || (q2 == r.ql && u < t)) ? 1u : 0u; }
                     res[pos] = r;
@@ -274,7 +293,7 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                 const uint32_t nmem = c1 - c0;
                 KJ_ROLLED
                 for (uint32_t wi = 0; wi < nmem; wi++) {
-                    const KjMatch sm = cls[wi == 0 ? c0 : c1 - wi];
+                    const Match sm = cls[wi == 0 ? c0 : c1 - wi];
                     const uint32_t mre1 = (uint32_t)sm.qi + sm.ql;         // match_right_end + 1
                     if (sm.qi > 0 && mre1 >= rp.m) {
                         const uint32_t new_len = mre1 < len ? mre1 : len;   // erase_pos (474)
@@ -293,11 +312,11 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                         const uint32_t okmask = w.ballot(ok); const uint32_t cnt = (uint32_t)kj_popc(okmask);
                         if (cnt) {
                             // the pop scans keys[0..n): squeeze out popped entries once the ring passes 64 slots and at least half are holes
-                            if (vq.n + cnt > rp.variant_cap || (vq.n + cnt > 64u && vq.live * 2u <= vq.n)) { kj_vq_compact(cx, vq); }
+                            if (vq.n + cnt > rp.variant_cap || (vq.n + cnt > 64u && vq.live * 2u <= vq.n)) { kj_vq_compact<LONG>(cx, vq); }
                             if (vq.n + cnt > rp.variant_cap) { if (w.lane == 0) kj_flag_error(cx, 4u); }
                             else {
                                 const uint32_t rk = (uint32_t)kj_popc(okmask & lanemask_lt(w.lane));
-                                KjVariant* V = vq.v + (vq.n + rk);                 // dereferenced by `ok` lanes only
+                                KjVariant<LONG>* V = vq.v + (vq.n + rk);           // dereferenced by `ok` lanes only
                                 // the parent's substitutions that survive the truncation, then the new one
                                 uint32_t ns = 0;
                                 KJ_ROLLED
@@ -307,10 +326,10 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                                 }
                                 if (ok) {
                                     V->subs[ns] = (pos << 5) | sub;
-                                    V->lo = (uint64_t)lo; V->hi = (uint64_t)hi; V->pay = kj_qpay(arr, true, start, new_len);
+                                    V->lo = (uint64_t)lo; V->hi = (uint64_t)hi; V->pay = kj_qpay<LONG>(arr, true, start, new_len);
                                     V->diff = diff + (int)tb.b62[o][sub] - (int)tb.b62[sub][sub];
-                                    V->matchlen = (uint16_t)(sm.ql + 1u); V->num_mm = (uint8_t)(ns + 1u); V->pad = 0; V->pad2 = 0;
-                                    vq.key(vq.n + rk) = kj_qkey((uint32_t)after, KJ_ORDER_LATE + q.late + rk);
+                                    V->matchlen = (PosT)(sm.ql + 1u); V->num_mm = (uint8_t)(ns + 1u); V->pad = 0; V->pad2 = 0;
+                                    vq.key(vq.n + rk) = kj_qkey<LONG>((uint32_t)after, (LONG ? KJ_ORDER_LATE_LONG : KJ_ORDER_LATE) + q.late + rk);
                                 }
                                 vq.n += cnt; vq.live += cnt; q.late += cnt;
 #if defined(KJ_EMU)
@@ -337,16 +356,16 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             // evaluation position of candidate t: non-heads keep their relative order, heads go last in reverse class order
             const uint32_t t = (uint32_t)w.lane;
             if (t < ncand) {
-                const KjMatch r = cls[t]; const bool head = (heads >> t) & 1u;
+                const Match r = cls[t]; const bool head = (heads >> t) & 1u;
                 const uint32_t cidx = (uint32_t)kj_popc(heads & ((2u << t) - 1u)) - 1u;           // class index of t
                 const uint32_t pos = head ? (ncand - K) + (K - 1u - cidx) : t - (cidx + 1u);
                 int sc = (int)pre[r.qi + r.ql] - (int)pre[r.qi] + diff; if (sc < 0) sc = 0;
-                res[pos].lo = r.lo | ((uint64_t)r.qi << 48); res[pos].len = r.len; res[pos].qi = (uint16_t)(sc > 65535 ? 65535 : sc); res[pos].ql = r.ql;      // (the match start rides in the free top bits of lo: the verbose output needs it)
+                res[pos].lo = r.lo | ((uint64_t)r.qi << QI_SHIFT); res[pos].len = r.len; res[pos].qi = LONG ? (PosT)sc : (PosT)(sc > 65535 ? 65535 : sc); res[pos].ql = r.ql;      // (the match start rides in the free top bits of lo: the verbose output needs it)
             }
             w.sync();
             // the sequential best-list update of the reference, closed form: the list ends up holding the entries that equal the final
             // maximum, in evaluation order, as long as fewer than 20 are held (a higher score empties the list first)
-            KjMatch e; e.lo = 0; e.len = 0; e.qi = 0; e.ql = 0; if (t < ncand) e = res[t];
+            Match e; e.lo = 0; e.len = 0; e.qi = 0; e.ql = 0; if (t < ncand) e = res[t];
             const uint32_t sc = t < ncand ? (uint32_t)e.qi : 0u; const bool valid = t < ncand && sc >= rp.min_score;
             const uint32_t mx = warp_max_u32(w, valid ? sc : 0u);
             if (mx > 0 && mx >= best) {
@@ -354,13 +373,13 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
                 const uint32_t eq = w.ballot(valid && sc == mx);
                 const uint32_t slot = nbest + (uint32_t)kj_popc(eq & lanemask_lt(w.lane));
                 const bool take = valid && sc == mx && slot < KJ_MAX_BEST_SI;
-                if (take) { bl[slot].lo = e.lo & 0xffffffffffffull; bl[slot].len = e.len; bl[slot].aux = 0; }
+                if (take) { bl[slot].lo = e.lo & LO_MASK; bl[slot].len = e.len; bl[slot].aux = 0; }
                 if (cx.text) {       // best_matches (ConsumerThread.cpp:779-790): the matched text of every entry of the best list, in list order
                     const uint32_t mylen = take ? (uint32_t)e.ql + 1u : 0u; const uint32_t endp = kj_scan_incl(w, mylen);
                     const uint32_t at = cx.text_len + endp - mylen, tot = w.shfl(endp, 31);
                     if (cx.text_len + tot > cx.text_cap) { if (w.lane == 0) kj_flag_error(cx, 128u); }
                     else {
-                        if (take) { const uint32_t qi0 = (uint32_t)(e.lo >> 48); for (uint32_t u = 0; u + 1u < mylen; u++) cx.text[at + u] = tb.letters[frag[qi0 + u]]; cx.text[at + mylen - 1u] = ','; }
+                        if (take) { const uint32_t qi0 = (uint32_t)(e.lo >> QI_SHIFT); for (uint32_t u = 0; u + 1u < mylen; u++) cx.text[at + u] = tb.letters[frag[qi0 + u]]; cx.text[at + mylen - 1u] = ','; }
                         cx.text_len += tot;
                     }
                 }
@@ -374,26 +393,26 @@ static KJ_DEV uint32_t kj_classify_greedy(KjWarpCtx& cx, KjQueue& q, double quer
             for (uint32_t b = 0; b < ncand; b += 32) {
                 uint32_t t = b + (uint32_t)w.lane;
                 if (t < ncand) {
-                    KjMatch r = cls[t]; bool head = (t == 0) || cls[t - 1].ql != r.ql;
+                    Match r = cls[t]; bool head = (t == 0) || cls[t - 1].ql != r.ql;
                     uint32_t cidx = 0, heads_before = 0;                   // class index of t, number of heads at indices < t
                     KJ_ROLLED
                     for (uint32_t u = 1; u <= t; u++) if (cls[u].ql != cls[u - 1].ql) cidx++;
                     heads_before = cidx + (head ? 0u : 1u);
                     uint32_t pos = head ? (ncand - K) + (K - 1u - cidx) : t - heads_before;
                     int sc = (int)pre[r.qi + r.ql] - (int)pre[r.qi] + diff; if (sc < 0) sc = 0;
-                    res[pos].lo = r.lo | ((uint64_t)r.qi << 48); res[pos].len = r.len; res[pos].qi = (uint16_t)(sc > 65535 ? 65535 : sc); res[pos].ql = r.ql;
+                    res[pos].lo = r.lo | ((uint64_t)r.qi << QI_SHIFT); res[pos].len = r.len; res[pos].qi = LONG ? (PosT)sc : (PosT)(sc > 65535 ? 65535 : sc); res[pos].ql = r.ql;
                 }
             }
             w.sync();
             KJ_ROLLED
             for (uint32_t t = 0; t < ncand; t++) {
-                const KjMatch r = res[t]; const uint32_t sc = r.qi;
+                const Match r = res[t]; const uint32_t sc = r.qi;
                 if (sc < rp.min_score) continue;
                 bool took = false;
-                if (sc > best) { best = sc; nbest = 0; cx.text_len = 0; if (w.lane == 0) { bl[0].lo = r.lo & 0xffffffffffffull; bl[0].len = r.len; bl[0].aux = 0; } nbest = 1; took = true; }
-                else if (sc == best && nbest < KJ_MAX_BEST_SI) { if (w.lane == 0) { bl[nbest].lo = r.lo & 0xffffffffffffull; bl[nbest].len = r.len; bl[nbest].aux = 0; } nbest++; took = true; }
+                if (sc > best) { best = sc; nbest = 0; cx.text_len = 0; if (w.lane == 0) { bl[0].lo = r.lo & LO_MASK; bl[0].len = r.len; bl[0].aux = 0; } nbest = 1; took = true; }
+                else if (sc == best && nbest < KJ_MAX_BEST_SI) { if (w.lane == 0) { bl[nbest].lo = r.lo & LO_MASK; bl[nbest].len = r.len; bl[nbest].aux = 0; } nbest++; took = true; }
                 if (took && cx.text) {
-                    const uint32_t at = kj_emit_text(w, cx.text, cx.text_len, cx.text_cap, frag + (uint32_t)(r.lo >> 48), 1u, r.ql, tb.letters);
+                    const uint32_t at = kj_emit_text(w, cx.text, cx.text_len, cx.text_cap, frag + (uint32_t)(r.lo >> QI_SHIFT), 1u, r.ql, tb.letters);
                     if (at == 0xffffffffu) { if (w.lane == 0) kj_flag_error(cx, 128u); } else cx.text_len = at;
                 }
             }

@@ -30,6 +30,7 @@
 #define KJ_CLAIM 4               // read items claimed per atomic by a warp
 #define KJ_CHUNK_READS (1u << 20)
 #define KJ_CHUNK_BYTES (1ull << 28)  // and at most this many bases of one mate per chunk (long reads)
+#define KJ_LONG_GAP 4096u        // short reads in a row that end a chunk of the long-read kernels (kj_classify: fewer run with it)
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { kj_err() = std::string(#call) + ": " + cudaGetErrorString(e_); return KJ_ERR_CUDA; } } while (0)
 
@@ -46,9 +47,20 @@ static __host__ __device__ __forceinline__ KjRunParams kj_fixed_profile(int mode
 // VB = true: the verbose outputs (id sets, accession sets, fragment strings) are compiled in; the kernels of the normal path carry none of it.
 // ROLE: 0 = the whole item in this kernel; 1 = front end only (translation, fragments, ranked queue -> a record per item in `prep`); 2 = search only (from the records).
 // Greedy runs as the pair 1 + 2 over sub-batches of the launch (kj_core.h: the search loop then shares the instruction cache with nothing it does not need).
-template <int MODE, class IdxT, bool GWS, bool FIX, bool VB, int ROLE>
-__global__ void __launch_bounds__(KJ_WARPS_PER_CTA * 32, MODE == 0 ? KJ_MIN_BLOCKS : ROLE != 0 ? KJ_MIN_BLOCKS_GREEDY_SPLIT : KJ_MIN_BLOCKS_GREEDY)
-kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ KjRunParams rp, const __grid_constant__ KjSmemLayout lay,
+// LONG = true: the long-read kernels (kj_classify_long_kernel; the work space in global memory, the general profile, ROLE 0).
+#define KJ_CLASSIFY_PARAMS const KjDevIndex* __restrict__ g_ix, const __grid_constant__ KjRunParams rp, const __grid_constant__ KjSmemLayout lay, \
+                   const uint8_t* __restrict__ seq1, const uint64_t* __restrict__ off1, \
+                   const uint8_t* __restrict__ seq2, const uint64_t* __restrict__ off2, \
+                   uint64_t base1, uint64_t base2, uint64_t n_reads, \
+                   uint64_t* __restrict__ taxon_out, uint32_t* __restrict__ best_out, uint64_t* __restrict__ ids_out, uint8_t* __restrict__ nids_out, uint32_t* __restrict__ compact_out, \
+                   unsigned long long* __restrict__ counter, KjKept* __restrict__ spill, uint8_t* __restrict__ gscratch, \
+                   uint32_t gscratch_bytes, uint8_t* __restrict__ gws, unsigned long long* __restrict__ counts, uint32_t* __restrict__ err, \
+                   uint32_t* __restrict__ acc_out, uint8_t* __restrict__ nacc_out, char* __restrict__ frag_out, uint32_t frag_stride, uint32_t* __restrict__ frag_len_out, \
+                   uint8_t* __restrict__ prep, uint32_t prep_stride, uint64_t r_begin
+#define KJ_CLASSIFY_ARGS g_ix, rp, lay, seq1, off1, seq2, off2, base1, base2, n_reads, taxon_out, best_out, ids_out, nids_out, compact_out, counter, spill, gscratch, \
+                   gscratch_bytes, gws, counts, err, acc_out, nacc_out, frag_out, frag_stride, frag_len_out, prep, prep_stride, r_begin
+template <int MODE, class IdxT, bool GWS, bool FIX, bool VB, int ROLE, bool LONG>
+static __device__ __forceinline__ void kj_classify_body(const KjDevIndex* __restrict__ g_ix, const KjRunParams& rp, const KjSmemLayout& lay,
                    const uint8_t* __restrict__ seq1, const uint64_t* __restrict__ off1,
                    const uint8_t* __restrict__ seq2, const uint64_t* __restrict__ off2,
                    uint64_t base1, uint64_t base2, uint64_t n_reads,
@@ -101,7 +113,7 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
             const uint8_t* p2 = paired ? seq2 + b0 : nullptr;
             uint32_t best = 0;
             if (VB && frag_out) { cx.text = frag_out + r * frag_stride; cx.text_len = 0; }
-            uint32_t t = kj_classify_item<MODE, IdxT, ROLE>(cx, p1, (int)(a1 - a0), p2, (int)(b1 - b0), paired, best, ROLE ? prep + (size_t)(r - r_begin) * prep_stride : nullptr);
+            uint32_t t = kj_classify_item<MODE, IdxT, ROLE, LONG>(cx, p1, (int)(a1 - a0), p2, (int)(b1 - b0), paired, best, ROLE ? prep + (size_t)(r - r_begin) * prep_stride : nullptr);
             if (ROLE == 1) { cx.w.sync(); continue; }
             const uint64_t id = t == KJ_TAX_BAD ? 0ull : sh->ix.tax_id[t];
             if (cx.w.lane == 0) {
@@ -136,6 +148,13 @@ kj_classify_kernel(const KjDevIndex* __restrict__ g_ix, const __grid_constant__ 
         }
     }
 }
+template <int MODE, class IdxT, bool GWS, bool FIX, bool VB, int ROLE>
+__global__ void __launch_bounds__(KJ_WARPS_PER_CTA * 32, MODE == 0 ? KJ_MIN_BLOCKS : ROLE != 0 ? KJ_MIN_BLOCKS_GREEDY_SPLIT : KJ_MIN_BLOCKS_GREEDY)
+kj_classify_kernel(KJ_CLASSIFY_PARAMS) { kj_classify_body<MODE, IdxT, GWS, FIX, VB, ROLE, false>(KJ_CLASSIFY_ARGS); }
+// mates longer than KJ_MAX_READ_LEN (kj_set_max_read_len): wide fields (kj_core.h KjW<true>); same signature, so the host launches it like the others
+template <int MODE, class IdxT, bool VB>
+__global__ void __launch_bounds__(KJ_WARPS_PER_CTA * 32, MODE == 0 ? KJ_MIN_BLOCKS : KJ_MIN_BLOCKS_GREEDY)
+kj_classify_long_kernel(KJ_CLASSIFY_PARAMS) { kj_classify_body<MODE, IdxT, true, false, VB, 0, true>(KJ_CLASSIFY_ARGS); }
 
 // Every instantiation has the same signature: the host picks one per launch (kj_select_kernel), sets it up and launches it through the pointer.
 using KjKernel = decltype(&kj_classify_kernel<0, uint32_t, false, false, false, 0>);
@@ -150,8 +169,16 @@ static KjKernel kj_select_kernel_t(bool gws, bool fixed, bool verbose, int role)
     }
     return kj_classify_kernel<MODE, T, false, false, false, 0>;
 }
-// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact (64-bit intervals; kj_layout.h)
-static KjKernel kj_select_kernel(int mode, int layout, bool gws, bool fixed, bool verbose, int role) {
+template <int MODE, class T>
+static KjKernel kj_select_long_kernel_t(bool verbose) { return verbose ? kj_classify_long_kernel<MODE, T, true> : kj_classify_long_kernel<MODE, T, false>; }
+// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact (64-bit intervals; kj_layout.h).  long_reads: the batch holds mates longer than
+// KJ_MAX_READ_LEN (only the work space in global memory, the general profile and ROLE 0 exist for them).
+static KjKernel kj_select_kernel(int mode, int layout, bool gws, bool fixed, bool verbose, int role, bool long_reads = false) {
+    if (long_reads) {
+        if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_long_kernel_t<0, KjCompactIdx>(verbose) : kj_select_long_kernel_t<1, KjCompactIdx>(verbose);
+        if (mode == 0) return layout ? kj_select_long_kernel_t<0, uint64_t>(verbose) : kj_select_long_kernel_t<0, uint32_t>(verbose);
+        return layout ? kj_select_long_kernel_t<1, uint64_t>(verbose) : kj_select_long_kernel_t<1, uint32_t>(verbose);
+    }
     if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_kernel_t<0, KjCompactIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjCompactIdx>(gws, fixed, verbose, role);
     if (mode == 0) return layout ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
     return layout ? kj_select_kernel_t<1, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<1, uint32_t>(gws, fixed, verbose, role);
@@ -215,6 +242,7 @@ struct KjSlot {
     KjDevBuf seq[2], off[2];                                        // staging of kj_classify (host buffers), one per mate
     KjDevBuf tax, best, ids, nids, acc, nacc, frag, fraglen;        // outputs of a chunk
     KjDevBuf spill, gscratch, ws;                                   // per-warp global scratch: spill entries, Greedy variant ring, work space of long reads
+    bool long_scratch = false;                                      // the scratch was sized by a launch of the long-read kernels (released by the next other launch)
     cudaStream_t stream = nullptr, fstream = nullptr;               // the slot's stream, and the front-end stream of the two-kernel Greedy path
     cudaEvent_t ev_in = nullptr, ev_f[2] = {nullptr, nullptr}, ev_s[2] = {nullptr, nullptr};     // hand-over events between the two
 };
@@ -235,6 +263,7 @@ struct kj_ctx {
     KjDevBuf evbreaks; uint32_t n_evbreaks = 0;
     KjDevBuf counts, counts_pending; uint32_t n_counts = 0, n_present = 0;   // per-taxon read counts (+1 slot: unclassified)
     uint32_t variant_boost = 1;    // Greedy variant-ring capacity multiplier, raised after an overflow (flag 4) so that a retry succeeds
+    uint32_t max_read_len = KJ_MAX_READ_LEN;    // longest mate admitted (kj_set_max_read_len); protein reads: a third of it
     KjDevBuf prep;                 // prepared-item records of the two-kernel Greedy path (two slots x two buffers)
     KjSlot slot[2];
     cudaEvent_t ev_a = nullptr, ev_b = nullptr;
@@ -449,6 +478,12 @@ extern "C" int kj_create_from_native(kj_ctx** out, int device, const kj_params* 
     return create_ctx(out, device, params, [&](KjHostIndex& H) { return kj_host_index_read(path, H); });
 }
 
+extern "C" int kj_set_max_read_len(kj_ctx* c, uint32_t bases) {
+    if (!c) { kj_err() = "kj_set_max_read_len: null argument"; return KJ_ERR_ARG; }
+    if (bases < KJ_MAX_READ_LEN || bases > KJ_MAX_LONG_READ_LEN) { kj_err() = "kj_set_max_read_len: the limit must lie in [KJ_MAX_READ_LEN, KJ_MAX_LONG_READ_LEN] = [16383, 1048575]"; return KJ_ERR_ARG; }
+    c->max_read_len = bases; return KJ_OK;
+}
+
 extern "C" int kj_set_params(kj_ctx* c, const kj_params* p) {
     if (!c || !p) { kj_err() = "kj_set_params: null argument"; return KJ_ERR_ARG; }
     int rc = kj_check_params(*p); if (rc) return rc;
@@ -469,31 +504,66 @@ extern "C" void kj_destroy(kj_ctx* c) {
     delete c;              // the device buffers go with their owners
 }
 
+// The grid of a long-read launch: per-warp scratch grows linearly with the longest read (about 100 MB per warp at 1 Mb), so the persistent grid is
+// cut to the CTAs whose scratch fits half of the free HBM (the other pipeline slot may need the same); this slot's current buffers count as free,
+// they are replaced.  A read is never spread over warps: if not even one CTA fits, the launch fails.
+static int long_read_grid(kj_ctx* c, const KjSlot& S, const KjRunParams& rp, size_t per_warp, int& grid) {
+    size_t fr = 0, to = 0; CK(cudaMemGetInfo(&fr, &to));
+    const size_t reserve = 256ull << 20, avail = fr + S.spill.cap + S.gscratch.cap + S.ws.cap;
+    size_t budget = avail > reserve ? (avail - reserve) / 2 : 0;
+    if (const char* v = getenv("KJ_LONG_BUDGET_MB")) budget = (size_t)atoll(v) << 20;      // test hook: a smaller budget
+    const size_t per_cta = per_warp * KJ_WARPS_PER_CTA, ctas = budget / per_cta;
+    if (ctas < 1) {
+        char b[240]; snprintf(b, sizeof b, "reads of up to %u bases need %zu bytes of work space per warp (%zu per CTA of %d warps); the budget of free device memory is %zu bytes",
+                              rp.max_len, per_warp, per_cta, KJ_WARPS_PER_CTA, budget);
+        kj_err() = b; return KJ_ERR_NOMEM;
+    }
+    if ((size_t)grid > ctas) grid = (int)ctas;
+    c->grid = grid; c->grid_kernel = nullptr;      // the geometry of this launch; the next launch derives its own
+    return KJ_OK;
+}
+
 // one launch over reads [0,n) whose sequences/offsets are resident on the device
 static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_off1, const uint8_t* d_seq2, const uint64_t* d_off2, uint64_t base1, uint64_t base2,
                   uint64_t n, uint32_t max1, uint32_t max2, const KjOut& o, cudaStream_t st, bool time_it) {
+    const bool raised = c->max_read_len != KJ_MAX_READ_LEN; char msg[200];
     if (c->params.input_is_protein) {
         if (d_seq2) { kj_err() = "protein input only supports one input (kaiju.cpp:201)"; return KJ_ERR_ARG; }
-        if (max1 > KJ_MAX_PROTEIN_LEN) { kj_err() = "protein read longer than KJ_MAX_PROTEIN_LEN (5461 residues) is not supported"; return KJ_ERR_UNSUPPORTED; }
-    } else if (max1 > KJ_MAX_READ_LEN || max2 > KJ_MAX_READ_LEN) { kj_err() = "read longer than KJ_MAX_READ_LEN (16383 bases) is not supported"; return KJ_ERR_UNSUPPORTED; }
+        if (max1 > c->max_read_len / 3) {
+            if (!raised) kj_err() = "protein read longer than KJ_MAX_PROTEIN_LEN (5461 residues) is not supported";
+            else { snprintf(msg, sizeof msg, "protein read longer than %u residues (a third of kj_set_max_read_len's %u bases) is not supported", c->max_read_len / 3, c->max_read_len); kj_err() = msg; }
+            return KJ_ERR_UNSUPPORTED;
+        }
+    } else if (max1 > c->max_read_len || max2 > c->max_read_len) {
+        if (!raised) kj_err() = "read longer than KJ_MAX_READ_LEN (16383 bases) is not supported";
+        else { snprintf(msg, sizeof msg, "read longer than %u bases (kj_set_max_read_len) is not supported", c->max_read_len); kj_err() = msg; }
+        return KJ_ERR_UNSUPPORTED;
+    }
+    // the kernel follows from the read lengths alone: mates beyond KJ_MAX_READ_LEN need the long-read kernels' wide fields
+    const bool long_reads = c->params.input_is_protein ? max1 > KJ_MAX_PROTEIN_LEN : std::max(max1, max2) > KJ_MAX_READ_LEN;
     KjRunParams rp; kj_fill_run_params(c->params, std::max(max1, max2), rp);
     rp.ev_breaks = c->evbreaks.as<double>(); rp.n_ev_breaks = c->n_evbreaks;
     rp.variant_cap *= c->variant_boost;
     const bool verbose = o.ids || o.acc || o.frag;
-    const KjSmemLayout lay = kj_smem_layout(rp);
+    const KjSmemLayout lay = long_reads ? kj_smem_layout<true>(rp) : kj_smem_layout(rp);
+    const uint32_t gs_bytes = long_reads ? kj_greedy_scratch_bytes<true>(rp) : kj_greedy_scratch_bytes(rp);
     const size_t head = kj_align((uint32_t)sizeof(KjCtaShared), 16), ws_smem = head + (size_t)KJ_WARPS_PER_CTA * lay.total;
-    rp.ws_global = ws_smem > KJ_SMEM_WS_LIMIT ? 1u : 0u;
+    rp.ws_global = long_reads || ws_smem > KJ_SMEM_WS_LIMIT ? 1u : 0u;
     const size_t smem = rp.ws_global ? head : ws_smem;
     const bool fixed = !verbose && kj_use_fixed(rp);
     // Greedy with the work space in shared memory: front-end kernel + search kernel over sub-batches (the records of a sub-batch live in d_prep)
     const bool split = rp.mode == 1 && !rp.ws_global && !verbose && !getenv("KJ_NO_SPLIT");
-    const KjKernel kern = kj_select_kernel(rp.mode, c->H.wide, rp.ws_global, fixed, verbose, split ? 2 : 0);
+    const KjKernel kern = kj_select_kernel(rp.mode, c->H.wide, rp.ws_global, fixed, verbose, split ? 2 : 0, long_reads);
     const KjKernel front = split ? kj_select_kernel(rp.mode, c->H.wide, false, fixed, false, 1) : nullptr;
     int rc = configure_launch(c, front, kern, smem); if (rc) return rc;
-    const int grid = c->grid;
+    int grid = c->grid;
     KjSlot& S = c->slot[slot];
+    // the scratch of a long-read launch (up to half of the free HBM) goes back when this slot next launches without long reads
+    if (S.long_scratch && !long_reads) { S.spill.reset(); S.gscratch.reset(); S.ws.reset(); }
+    S.long_scratch = long_reads;
+    if (long_reads && (rc = long_read_grid(c, S, rp, (size_t)lay.total + (size_t)rp.scratch_entries * sizeof(KjKept) + gs_bytes, grid))) return rc;
     const size_t warps = (size_t)grid * KJ_WARPS_PER_CTA;
-    if ((rc = S.spill.grow(warps * rp.scratch_entries * sizeof(KjKept))) || (rc = S.gscratch.grow(warps * (size_t)kj_greedy_scratch_bytes(rp))) ||
+    if ((rc = S.spill.grow(warps * rp.scratch_entries * sizeof(KjKept))) || (rc = S.gscratch.grow(warps * (size_t)gs_bytes)) ||
         (rc = S.ws.grow(rp.ws_global ? warps * (size_t)lay.total : 0))) return rc;
     if (time_it) CK(cudaEventRecord(c->ev_a, st));
     const KjDevIndex* dix = (rp.mode == 0 && c->ix_mem.p && rp.m >= (uint32_t)c->kmer_k_mem) ? c->ix_mem.as<KjDevIndex>() : c->ix.as<KjDevIndex>();
@@ -516,7 +586,7 @@ static int launch(kj_ctx* c, int slot, const uint8_t* d_seq1, const uint64_t* d_
     auto run = [&](KjKernel k, cudaStream_t s, unsigned long long* ctr, uint8_t* pbuf, uint64_t b0, uint64_t b1) -> int {
         CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), s));
         k<<<grid, KJ_WARPS_PER_CTA * 32, smem, s>>>(dix, rp, lay, d_seq1, d_off1, d_seq2, d_off2, base1, base2, b1, o.tax, o.best, o.ids, o.nids, o.compact,
-                                                     ctr, S.spill.as<KjKept>(), S.gscratch.as<uint8_t>(), kj_greedy_scratch_bytes(rp), rp.ws_global ? S.ws.as<uint8_t>() : nullptr,
+                                                     ctr, S.spill.as<KjKept>(), S.gscratch.as<uint8_t>(), gs_bytes, rp.ws_global ? S.ws.as<uint8_t>() : nullptr,
                                                      o.counts, c->err.as<uint32_t>(), o.acc, o.nacc, o.frag, o.frag_stride, o.fraglen, pbuf, pstride, b0);
         c->launches++;
         return KJ_OK;
@@ -591,16 +661,20 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
     if (n == 0) return KJ_OK;
     CK(cudaSetDevice(c->device));
     const bool paired = seq2 != nullptr;
-    // batch-wide length bounds (fixes the shared-memory carve-up for all chunks)
-    uint32_t max1 = 0, max2 = 0;
+    // batch-wide length bounds (fix the shared-memory carve-up for all chunks): of all reads, and of the reads the short kernels take; and the
+    // reads that need the long-read kernels (a mate above KJ_MAX_READ_LEN bases, protein: KJ_MAX_PROTEIN_LEN residues), in input order
+    uint32_t max1 = 0, max2 = 0, smax1 = 0, smax2 = 0; std::vector<uint64_t> longs;
     {
-        unsigned nthr = std::max(1u, std::min(64u, std::thread::hardware_concurrency())); if (n < 65536) nthr = 1; std::vector<uint32_t> m1(nthr, 0), m2(nthr, 0); std::vector<std::thread> th;
-        for (unsigned t = 0; t < nthr; t++) th.emplace_back([&, t] { uint64_t a = n * t / nthr, b = n * (t + 1) / nthr; uint32_t x = 0, y = 0;
+        const uint32_t lim = c->params.input_is_protein ? KJ_MAX_PROTEIN_LEN : KJ_MAX_READ_LEN;
+        unsigned nthr = std::max(1u, std::min(64u, std::thread::hardware_concurrency())); if (n < 65536) nthr = 1;
+        std::vector<uint32_t> m1(nthr, 0), m2(nthr, 0), s1(nthr, 0), s2(nthr, 0); std::vector<std::vector<uint64_t>> lg(nthr); std::vector<std::thread> th;
+        for (unsigned t = 0; t < nthr; t++) th.emplace_back([&, t] { uint64_t a = n * t / nthr, b = n * (t + 1) / nthr; uint32_t x = 0, y = 0, sx = 0, sy = 0;
             for (uint64_t i = a; i < b; i++) { uint64_t l = off1[i + 1] - off1[i]; if (l > 0xffffffffull) l = 0xffffffffull; x = std::max(x, (uint32_t)l);
-                                               if (paired) { uint64_t k = off2[i + 1] - off2[i]; if (k > 0xffffffffull) k = 0xffffffffull; y = std::max(y, (uint32_t)k); } }
-            m1[t] = x; m2[t] = y; });
+                                               uint64_t k = 0; if (paired) { k = off2[i + 1] - off2[i]; if (k > 0xffffffffull) k = 0xffffffffull; y = std::max(y, (uint32_t)k); }
+                                               if (l > lim || k > lim) lg[t].push_back(i); else { sx = std::max(sx, (uint32_t)l); sy = std::max(sy, (uint32_t)k); } }
+            m1[t] = x; m2[t] = y; s1[t] = sx; s2[t] = sy; });
         for (auto& x : th) x.join();
-        for (unsigned t = 0; t < nthr; t++) { max1 = std::max(max1, m1[t]); max2 = std::max(max2, m2[t]); }
+        for (unsigned t = 0; t < nthr; t++) { max1 = std::max(max1, m1[t]); max2 = std::max(max2, m2[t]); smax1 = std::max(smax1, s1[t]); smax2 = std::max(smax2, s2[t]); longs.insert(longs.end(), lg[t].begin(), lg[t].end()); }
     }
     CK(cudaMemset(c->counts_pending.p, 0, (size_t)c->n_counts * 8));                // counts of this call: committed only if the whole call succeeds
     uint64_t chunk_reads = KJ_CHUNK_READS;
@@ -632,6 +706,20 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
             if (paired) { const uint64_t* e2p = std::upper_bound(off2 + start + 1, off2 + start + cnt + 1, off2[start] + KJ_CHUNK_BYTES); lim = std::min(lim, std::max<uint64_t>(1, (uint64_t)(e2p - (off2 + start + 1)))); }
             cnt = std::min(cnt, lim);
         }
+        // Reads that need the long-read kernels run in chunks of their own, so that the short reads of the call keep the short kernels and their
+        // full grid: a chunk is either a stretch without long reads, or it starts at a long read (or at fewer than KJ_LONG_GAP short reads before
+        // one) and ends where KJ_LONG_GAP short reads in a row follow; the few short reads inside it run on the long kernels with the same results.
+        bool long_chunk = false;
+        if (!longs.empty()) {
+            auto it = std::lower_bound(longs.begin(), longs.end(), start);
+            const uint64_t nl = it == longs.end() ? n : *it;
+            if (nl == n || nl - start >= KJ_LONG_GAP) cnt = std::min(cnt, nl - start);
+            else {
+                long_chunk = true; uint64_t e = nl + 1;
+                for (auto jt = it + 1; e - start < cnt; ++jt) { const uint64_t nx = jt == longs.end() ? n : *jt; if (nx == n || nx - e >= KJ_LONG_GAP) break; e = nx + 1; }
+                cnt = std::min(cnt, e - start);
+            }
+        }
         CK(cudaStreamSynchronize(st));                      // slot s free again (its previous D2H has landed)
         if (trace) { Tr t; for (auto& e : t.e) cudaEventCreate(&e); t.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - th0).count(); t.cnt = 0; tr.push_back(t); cudaEventRecord(tr.back().e[0], st); }
         const uint64_t b1 = off1[start], e1 = off1[start + cnt], b2 = paired ? off2[start] : 0, e2 = paired ? off2[start + cnt] : 0;
@@ -651,7 +739,7 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
         if (o.frag) { d.frag = S.frag.as<char>(); d.fraglen = S.fraglen.as<uint32_t>(); }
         d.frag_stride = o.frag_stride; d.counts = c->counts_pending.as<unsigned long long>();
         if ((rc = launch(c, (int)(k & 1), S.seq[0].as<uint8_t>(), S.off[0].as<uint64_t>(), paired ? S.seq[1].as<uint8_t>() : nullptr, paired ? S.off[1].as<uint64_t>() : nullptr,
-                         b1, b2, cnt, max1, max2, d, st, true))) return rc;
+                         b1, b2, cnt, long_chunk ? max1 : smax1, long_chunk ? max2 : smax2, d, st, true))) return rc;
         if (trace) cudaEventRecord(tr.back().e[2], st);
         CK(cudaMemcpyAsync(o.tax + start, d.tax, cnt * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         if (o.best) CK(cudaMemcpyAsync(o.best + start, d.best, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));

@@ -263,11 +263,21 @@ int kj_build_host_meta(const kj_index_view& v, const kj_taxonomy_view& t, uint32
     if (v.seq_accession && copies == 1) H.seq_acc.assign(v.seq_accession, v.seq_accession + v.nseq);
     H.sa_exp = v.chpt_exp; H.sa_check = (1ull << v.chpt_exp) - 1ull;                         // suffixArray_set_masks (suffixArray.c:34-37)
     H.sa_bias = ((int64_t)((int64_t)H.nseq - 1) >> v.chpt_exp) + 1;                          // bwt.c:115-116
-    // ---- ln(n!) exactly as the reference's literals (blast_seg.c:53-1306 are "%.6f" prints of lgamma)
-    H.lnfact.resize(10001);                                             // the reference's table lnfact[0..10000] (blast_seg.c:53-1306)
-    for (int i = 0; i < 10001; i++) { char b[64]; snprintf(b, sizeof b, "%.6f", lgamma((double)i + 1.0)); H.lnfact[(size_t)i] = strtod(b, nullptr); }
-    H.lnfact[0] = H.lnfact[1] = 0.0;
+    kj_lnfact_table(H.lnfact);
     return KJ_OK;
+}
+
+// ln(n!) exactly as the reference's s_lnfact (blast_seg.c:1852-1856): its table lnfact[0..10000] ("%.6f" prints of lgamma, blast_seg.c:53-1306), and
+// Stirling's formula above it.  The long-read kernels trim SEG regions of up to a fragment's length, so the table runs to the longest fragment of a
+// KJ_MAX_LONG_READ_LEN read; the first KJ_LNFACT_REF entries are the only ones a device-native index file stores.
+void kj_lnfact_table(std::vector<double>& t) {
+    const size_t had = t.size() >= KJ_LNFACT_REF ? KJ_LNFACT_REF : 0;
+    t.resize(KJ_LNFACT_LEN);
+    if (!had) {
+        for (int i = 0; i < KJ_LNFACT_REF; i++) { char b[64]; snprintf(b, sizeof b, "%.6f", lgamma((double)i + 1.0)); t[(size_t)i] = strtod(b, nullptr); }
+        t[0] = t[1] = 0.0;
+    }
+    for (int n = KJ_LNFACT_REF; n < KJ_LNFACT_LEN; n++) t[(size_t)n] = ((n + 0.5) * log((double)n) - n + 0.9189385332);
 }
 
 int kj_build_host_index(const kj_index_view& v, const kj_taxonomy_view& t, KjHostIndex& H) {
@@ -477,7 +487,7 @@ template <class T> uint64_t mix_vec(uint64_t h, const std::vector<T>& v) { retur
 uint64_t index_checksum(const KjHostIndex& H) {
     uint64_t h = 0x6b616a755f623230ull;
     h = mix_bytes(h, &H.tables, sizeof(KjTables)); h = mix_vec(h, H.rank); h = mix_vec(h, H.letters); h = mix_vec(h, H.sa_tax); h = mix_vec(h, H.seq_tax);
-    h = mix_vec(h, H.tax_parent); h = mix_vec(h, H.tax_depth); h = mix_vec(h, H.tax_id); h = mix_vec(h, H.lnfact); h = mix_vec(h, H.kmer); h = mix_vec(h, H.kmer32);
+    h = mix_vec(h, H.tax_parent); h = mix_vec(h, H.tax_depth); h = mix_vec(h, H.tax_id); h = mix_bytes(h, H.lnfact.data(), std::min<size_t>(H.lnfact.size(), KJ_LNFACT_REF) * sizeof(double)); h = mix_vec(h, H.kmer); h = mix_vec(h, H.kmer32);
     return h;
 }
 template <class T> bool put(FILE* f, const std::vector<T>& v) { return v.empty() || fwrite(v.data(), sizeof(T), v.size(), f) == v.size(); }
@@ -491,11 +501,11 @@ int kj_host_index_write(const KjHostIndex& H, const char* path) {
     h.version = kNativeVersion; h.sizeof_tables = (uint32_t)sizeof(KjTables); h.sizeof_rank = 8u * kj_rank_words(H.wide); h.alen = (uint32_t)H.alen;
     h.nb = H.nb; h.bwtlen = H.bwtlen; memcpy(h.C, H.C, sizeof h.C); h.sa_check = H.sa_check; h.sa_bias = H.sa_bias; h.sa_exp = H.sa_exp; h.nseq = H.nseq; h.n_present = H.n_present;
     h.kmer_k = H.kmer_k; h.wide = H.wide; h.db_length = H.db_length; h.quirk_lo = H.quirk_lo; memcpy(h.quirk_d, H.quirk_d, sizeof h.quirk_d);
-    h.n_rank = H.rank.size(); h.n_letters = H.letters.size(); h.n_sa_tax = H.sa_tax.size(); h.n_seq_tax = H.seq_tax.size(); h.n_tax = H.tax_id.size(); h.n_lnfact = H.lnfact.size();
+    h.n_rank = H.rank.size(); h.n_letters = H.letters.size(); h.n_sa_tax = H.sa_tax.size(); h.n_seq_tax = H.seq_tax.size(); h.n_tax = H.tax_id.size(); h.n_lnfact = std::min<size_t>(H.lnfact.size(), KJ_LNFACT_REF);
     h.n_kmer = H.kmer.size(); h.n_kmer32 = H.kmer32.size(); h.checksum = index_checksum(H);
     bool ok = fwrite(kNativeMagic, 1, 8, f) == 8 && fwrite(&h, sizeof h, 1, f) == 1 && fwrite(&H.tables, sizeof(KjTables), 1, f) == 1 &&
               put(f, H.rank) && put(f, H.letters) && put(f, H.sa_tax) && put(f, H.seq_tax) && put(f, H.tax_parent) && put(f, H.tax_depth) && put(f, H.tax_id) &&
-              put(f, H.lnfact) && put(f, H.kmer) && put(f, H.kmer32);
+              fwrite(H.lnfact.data(), sizeof(double), h.n_lnfact, f) == h.n_lnfact && put(f, H.kmer) && put(f, H.kmer32);
     ok = (fclose(f) == 0) && ok;
     if (!ok) { kj_err() = std::string("write error on ") + path; return KJ_ERR_IO; }
     return KJ_OK;
@@ -518,6 +528,7 @@ int kj_host_index_read(const char* path, KjHostIndex& H) {
     char extra; const bool at_end = fread(&extra, 1, 1, f) == 0;
     fclose(f);
     if (!ok || !at_end || h.n_present > h.n_tax || index_checksum(H) != h.checksum) { kj_err() = std::string(path) + " is truncated or corrupt"; return KJ_ERR_IO; }
+    kj_lnfact_table(H.lnfact);                                          // the file holds the reference's table; Stirling's values above it
     // internal consistency (a crafted file with a recomputed checksum must not lead to out-of-bounds reads on the device)
     uint64_t nk = 1; for (int d = 0; d < H.kmer_k; d++) nk *= 20;
     bool good = H.bwtlen > 0 && H.bwtlen < (1ull << 38) && h.n_letters >= H.bwtlen / KJ_LETTERS_PER_WORD + 1 && h.n_seq_tax == H.nseq && H.sa_exp >= 0 && H.sa_exp <= 30 &&

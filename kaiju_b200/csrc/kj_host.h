@@ -53,3 +53,6 @@ int kj_check_params(const kj_params& p);
 int kj_build_evalue_breaks(const kj_params& p, double db_length, std::vector<double>& breaks);
 // per-warp scratch geometry for a batch whose longest mate has max_len bases
 void kj_fill_run_params(const kj_params& p, uint32_t max_len, KjRunParams& rp);
+#define KJ_LNFACT_REF 10001                                  // entries of the reference's ln(n!) table (blast_seg.c:53-1306)
+#define KJ_LNFACT_LEN (KJ_MAX_LONG_READ_LEN / 3 + 16)        // ln(n!) for every SEG region length of a KJ_MAX_LONG_READ_LEN read
+void kj_lnfact_table(std::vector<double>& t);

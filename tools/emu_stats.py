@@ -23,7 +23,7 @@ fmi, nodes = d + "/db.fmi", d + "/nodes.dmp"
 s1, o1, s2, o2 = db.reads(301, 0, n, 150, True)
 orc = Oracle(fmi, nodes)
 names = ["rounds", "round_steps", "lane_steps", "chains", "blocks", "lookaheads", "pops_frag", "pops_var", "var_steps", "var_pushed",
-         "id_reads", "kept", "sa_waves", "sa_lf_steps", "sa_dep_steps"]
+         "id_reads", "kept", "sa_waves", "sa_lf_steps", "sa_dep_steps", "lq_tops", "lq_slots"]
 for kw in (dict(mode="mem"), dict(mode="greedy")):
     P = make_params(**kw); kp = KjParams(**P); h = E.kjemu_create(fmi.encode(), nodes.encode(), C.byref(kp))
     have_array = E.kjemu_use_row_tax(h, 1)          # built once here (it also appends the suffix array's guard entry, as the device does)
