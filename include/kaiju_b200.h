@@ -108,7 +108,18 @@ int kj_create(kj_ctx **out, int device, const kj_params *params, const kj_index_
  * suffix sort.  With all copies carrying the taxon of their original, MEM results equal those on the base index; it exists to bring
  * indexes of 1e10 rows and more (~47 GB in HBM per 1e10 rows) onto a GPU for capacity and throughput measurements.  copies = 1 == kj_create. */
 int kj_create_scaled(kj_ctx **out, int device, const kj_params *params, const kj_index_view *index, const kj_taxonomy_view *taxonomy, uint32_t copies);
-double kj_index_build_ms(const kj_ctx *ctx);      /* wall time of the index construction inside kj_create / kj_create_scaled */
+/* kj_create_tiered: kj_create_scaled for indexes larger than the HBM of one GPU.  host_bytes is the most pinned host memory the index may take;
+ * the library alone decides whether anything goes there and how much.  Only a compact index whose construction does not fit in the HBM free
+ * at creation gets a host tier (mapped pinned host memory the kernels read over PCIe), placed in this order:
+ *   1. the suffix-array taxon and accession arrays (read once at the end of each suffix-array walk); the layout stays 2 (compact);
+ *   2. if that is not enough, also the tail of the compact rank records, so that 4 GB of HBM stay free for classification: layout 3.
+ * The superblock table, the k-mer table and the taxonomy stay in HBM.  Results are identical to those of an index held in HBM alone.  If the
+ * host tier would exceed host_bytes, KJ_ERR_NOMEM before any large allocation, and kj_last_error() names the HBM free, the host bytes needed
+ * and the budget.  The pinned memory is held until kj_destroy; pinning it counts in kj_index_build_ms.  host_bytes = 0 is kj_create_scaled
+ * (kj_create for copies = 1); indexes that fit in HBM are built exactly as there. */
+int kj_create_tiered(kj_ctx **out, int device, const kj_params *params, const kj_index_view *index, const kj_taxonomy_view *taxonomy,
+                     uint32_t copies, uint64_t host_bytes);
+double kj_index_build_ms(const kj_ctx *ctx);      /* wall time of the index construction inside kj_create / kj_create_scaled / kj_create_tiered */
 /* Device-native index file (SURVEY.md 8f-4): kj_native_index_write() transcodes once (the .fmi + nodes.dmp views as for kj_create) and
  * stores the arrays exactly as they are uploaded (one-hot rank records, packed letters, taxon-reduced suffix array, re-indexed
  * taxonomy, k-mer table); kj_create_from_native() then needs one sequential read and the upload -- no transcode at load time.
@@ -225,10 +236,12 @@ int kj_check_errors(kj_ctx *ctx);
 const char *kj_last_error(void);                  /* thread-local text of the last failure          */
 uint64_t kj_kernel_launches(const kj_ctx *ctx);   /* number of kernels this context has launched    */
 uint64_t kj_index_bytes(const kj_ctx *ctx);       /* bytes of HBM held by the index                 */
+uint64_t kj_index_host_bytes(const kj_ctx *ctx);  /* bytes of pinned host memory held by the index (its host tier, kj_create_tiered; else 0) */
 /* Rank layout of the context's index: 0 narrow (< 2^32 rows, 5.25 B per row), 1 wide (64-bit intervals, 3.5 B per row plus 0.67 B of packed
- * letters), 2 compact (64-bit intervals, 1.003 B per row, letters included).  A 64-bit index is built wide when the wide construction fits in
- * the HBM free at creation, else compact; when neither fits, kj_create / kj_create_scaled fail with KJ_ERR_NOMEM and kj_last_error() names the
- * bytes needed and the bytes free.  -1 for a null context. */
+ * letters), 2 compact (64-bit intervals, 1.003 B per row, letters included), 3 compact with its records split between HBM and host memory
+ * (kj_create_tiered).  A 64-bit index is built wide when the wide construction fits in the HBM free at creation, else compact; when neither
+ * fits, kj_create / kj_create_scaled fail with KJ_ERR_NOMEM and kj_last_error() names the bytes needed and the bytes free (kj_create_tiered:
+ * see there).  -1 for a null context. */
 int kj_index_layout(const kj_ctx *ctx);
 double kj_last_kernel_ms(const kj_ctx *ctx);      /* device time of the last classify kernel (CUDA events) */
 int kj_launch_geometry(const kj_ctx *ctx, int *grid, int *block, int *dyn_smem_bytes);  /* of the last classify launch */

@@ -85,6 +85,9 @@ def lib():
                                          C.c_void_p, C.c_void_p, C.c_void_p]
         L.kj_kernel_launches.restype = C.c_uint64; L.kj_kernel_launches.argtypes = [C.c_void_p]
         L.kj_index_bytes.restype = C.c_uint64; L.kj_index_bytes.argtypes = [C.c_void_p]
+        if hasattr(L, "kj_create_tiered"):
+            L.kj_create_tiered.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(KjParams), C.POINTER(KjIndexView), C.POINTER(KjTaxonomyView), C.c_uint32, C.c_uint64]
+            L.kj_index_host_bytes.restype = C.c_uint64; L.kj_index_host_bytes.argtypes = [C.c_void_p]
         if hasattr(L, "kj_index_layout"):
             L.kj_index_layout.restype = C.c_int; L.kj_index_layout.argtypes = [C.c_void_p]
         L.kj_last_kernel_ms.restype = C.c_double; L.kj_last_kernel_ms.argtypes = [C.c_void_p]
@@ -184,17 +187,18 @@ class Classifier:
     """One GPU context: the .fmi index and nodes.dmp taxonomy resident in HBM + run parameters.
     `Classifier(native_path, None)` loads a device-native index file written by write_native_index()."""
 
-    def __init__(self, fmi_path, nodes_path, device=0, params=None, copies=1, max_read_len=None, **kw):
+    def __init__(self, fmi_path, nodes_path, device=0, params=None, copies=1, max_read_len=None, host_memory=0, **kw):
         """copies > 1: the index of the collection in which every sequence occurs `copies` times (kj_create_scaled).
-        max_read_len: admit mates of up to this many bases (see set_max_read_len); None keeps the default, MAX_READ_LEN."""
-        self._init(fmi_path, nodes_path, device, params, copies, **kw)
+        max_read_len: admit mates of up to this many bases (see set_max_read_len); None keeps the default, MAX_READ_LEN.
+        host_memory: bytes of pinned host memory the index may take when it does not fit in HBM (kj_create_tiered); 0 = HBM only."""
+        self._init(fmi_path, nodes_path, device, params, copies, host_memory, **kw)
         if max_read_len is not None:
             try:
                 self.set_max_read_len(max_read_len)
             except Exception:
                 self.close(); raise
 
-    def _init(self, fmi_path, nodes_path, device, params, copies, **kw):
+    def _init(self, fmi_path, nodes_path, device, params, copies, host_memory=0, **kw):
         L = lib()
         self._ctx = C.c_void_p()
         if nodes_path is None:
@@ -212,7 +216,9 @@ class Classifier:
                 self.params = params if params is not None else make_params(**kw)
                 self.bwtlen = int(iv.bwtlen); self.nseq = int(iv.nseq)
                 self.bwtlen *= int(copies); self.nseq *= int(copies)
-                if int(copies) == 1:
+                if int(host_memory) > 0:
+                    _check(L.kj_create_tiered(C.byref(self._ctx), device, C.byref(self.params), C.byref(iv), C.byref(tv), int(copies), int(host_memory)))
+                elif int(copies) == 1:
                     _check(L.kj_create(C.byref(self._ctx), device, C.byref(self.params), C.byref(iv), C.byref(tv)))
                 else:
                     _check(L.kj_create_scaled(C.byref(self._ctx), device, C.byref(self.params), C.byref(iv), C.byref(tv), int(copies)))
@@ -332,8 +338,13 @@ class Classifier:
 
     @property
     def layout(self):
-        """Rank layout of the index in HBM: 0 narrow, 1 wide, 2 compact (kj_index_layout)."""
+        """Rank layout of the index: 0 narrow, 1 wide, 2 compact, 3 compact with records in host memory (kj_index_layout)."""
         return int(lib().kj_index_layout(self._ctx))
+
+    @property
+    def host_bytes(self):
+        """Bytes of pinned host memory held by the index (its host tier; 0 unless created with host_memory)."""
+        return int(lib().kj_index_host_bytes(self._ctx))
 
     @property
     def index_build_ms(self):

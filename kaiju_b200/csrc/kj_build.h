@@ -182,9 +182,17 @@ static int kj_bld_upload(void* d, const void* h, size_t bytes) {
 // ---- compact layout (kj_layout.h): one CTA per 65536-row superblock, one thread per 128-row record.  A record depends only on its own
 // superblock, so the BWT can be built a chunk of whole superblocks at a time.  `bwt` holds rows [row0, ...) (rep == 1) or the whole base BWT
 // (rep > 1: row r of the K-fold index is base row r / K).  sb_tot[s][c] = #c in superblock s (KJ_CSB_STRIDE per superblock).
+// Record b goes to `dev` below the split record nb_dev, else to `host` (the host tier of kj_create_tiered: pinned host memory mapped into the
+// device's address space).  The build writes the host tier directly through the mapped pointer rather than staging it in HBM and copying: the
+// stores are posted PCIe writes of whole 16-byte words, each byte is written once, and no HBM is needed for a staging buffer -- HBM is exactly
+// what an index with a host tier lacks.
 #define KJ_CSB_RECS (1u << (KJ_CSB_SHIFT - 7))
+static __device__ __forceinline__ uint64_t* kj_bld_crec(uint64_t* dev, uint64_t* host, uint64_t nb_dev, uint64_t b) {
+    return b < nb_dev ? dev + b * KJ_RANK_WORDS_COMPACT : host + (b - nb_dev) * KJ_RANK_WORDS_COMPACT;
+}
 __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* __restrict__ bwt, const __grid_constant__ KjBuildLcode lc, uint64_t s0, uint64_t row0, uint64_t n,
-                                                                  uint32_t rep, uint64_t nb, uint64_t* __restrict__ rec_out, uint32_t* __restrict__ sb_tot) {
+                                                                  uint32_t rep, uint64_t nb, uint64_t* __restrict__ rec_out, uint64_t* __restrict__ rec_host, uint64_t nb_dev,
+                                                                  uint32_t* __restrict__ sb_tot) {
     __shared__ uint8_t lcs[256];
     __shared__ __align__(16) uint16_t cnt[KJ_CSB_RECS][KJ_MAX_ALEN];    // #c in the first half of each record, then the midpoint counts
     __shared__ uint8_t full[KJ_CSB_RECS][KJ_MAX_ALEN];                  // #c in each record
@@ -208,7 +216,7 @@ __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* 
             }
             pw[5 * h] = p0; pw[5 * h + 1] = p1; pw[5 * h + 2] = p2; pw[5 * h + 3] = p3; pw[5 * h + 4] = p4;
         }
-        ulonglong2* o = (ulonglong2*)(rec_out + b * KJ_RANK_WORDS_COMPACT);
+        ulonglong2* o = (ulonglong2*)kj_bld_crec(rec_out, rec_host, nb_dev, b);
         #pragma unroll
         for (int q = 0; q < 5; q++) o[q] = make_ulonglong2(pw[2 * q], pw[2 * q + 1]);
     }
@@ -222,7 +230,7 @@ __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* 
     for (uint32_t r = threadIdx.x; r < KJ_CSB_RECS; r += KJ_BLD_THREADS) {
         const uint64_t b = (s << (KJ_CSB_SHIFT - 7)) + r;
         if (b >= nb) break;
-        const ulonglong2* src = (const ulonglong2*)&cnt[r][0]; ulonglong2* o = (ulonglong2*)(rec_out + b * KJ_RANK_WORDS_COMPACT + KJ_CPT_COUNT_WORD);
+        const ulonglong2* src = (const ulonglong2*)&cnt[r][0]; ulonglong2* o = (ulonglong2*)(kj_bld_crec(rec_out, rec_host, nb_dev, b) + KJ_CPT_COUNT_WORD);
         #pragma unroll
         for (int q = 0; q < 3; q++) o[q] = src[q];
     }
@@ -246,8 +254,9 @@ static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBu
     KjHostIndex& H = c->H; const int alen = H.alen; const uint64_t n = H.bwtlen, nb = H.nb, nsb = kj_csb_count(n);
     const uint64_t CH = kj_compact_chunk_rows(), sb_per_chunk = CH >> KJ_CSB_SHIFT;
     int rc; KjDevBuf bwt, sbt, small;
-    if ((rc = c->rank.grow(nb * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
-    tot += nb * KJ_RANK_WORDS_COMPACT * 8 + nsb * KJ_CSB_STRIDE * 8;
+    const uint64_t nd = c->nb_dev;                      // records [nd, nb) go to the host tier (kj_choose_layout)
+    if ((rc = c->rank.grow(nd * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->rank_host.grow((nb - nd) * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
+    tot += nd * KJ_RANK_WORDS_COMPACT * 8 + nsb * KJ_CSB_STRIDE * 8; c->host_bytes += (nb - nd) * KJ_RANK_WORDS_COMPACT * 8;
     if ((rc = sbt.grow(nsb * KJ_CSB_STRIDE * 4)) || (rc = small.grow(3 * KJ_MAX_ALEN * 8 + 64))) return rc;
     uint64_t* d_tot = small.as<uint64_t>(); uint64_t* d_C = d_tot + KJ_MAX_ALEN + 1;
     if (rep == 1) { if ((rc = bwt.grow((size_t)std::min(CH, n)))) return rc; }
@@ -255,7 +264,7 @@ static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBu
     for (uint64_t s0 = 0; s0 < nsb; s0 += sb_per_chunk) {
         const uint64_t row0 = s0 << KJ_CSB_SHIFT, nsc = std::min(sb_per_chunk, nsb - s0);
         if (rep == 1 && row0 < n) CK(cudaMemcpy(bwt.p, v.bwt + row0, (size_t)(std::min(n, row0 + CH) - row0), cudaMemcpyHostToDevice));
-        kj_bld_compact<<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, c->rank.as<uint64_t>(), sbt.as<uint32_t>());
+        kj_bld_compact<<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, c->rank.as<uint64_t>(), c->rank_host.as<uint64_t>(), nd, sbt.as<uint32_t>());
         CK(cudaGetLastError()); c->launches++;
         if (rep == 1) CK(cudaDeviceSynchronize());          // the next chunk's upload overwrites the staging buffer
     }
@@ -271,11 +280,22 @@ static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBu
     return KJ_OK;
 }
 
+// HBM the placement of kj_create_tiered leaves free next to an index with a host tier, for classification: the two pipeline slots' staging and
+// outputs for chunks of 2^20 read pairs (~0.7 GB), the per-warp spill, variant-ring and work-space scratch of the persistent grid (~0.3 GB for
+// PE150 on 132 SMs x 4 CTAs x 8 warps), the Greedy path's prepared-item buffers (4 x 1/16 of the free memory, at least 1 GB at this size) and the
+// CUDA context's own allocations, with room to spare for a read set that needs more scratch than PE150.
+#define KJ_TIER_HEADROOM (4ull << 30)
 // Layout of a 64-bit index built on the device: wide exactly when the peak HBM of the wide construction fits in the memory free now, else
 // compact; when the compact construction does not fit either, KJ_ERR_NOMEM before anything large is allocated.  A peak is the maximum over the
 // construction's phases: (1) BWT staging + scratch + the rank arrays, (2) rank arrays + suffix-array arrays + the upload chunk of the sampled
 // suffix array, (3) rank arrays + suffix-array arrays + the two level buffers of the k-mer table.
-static int kj_choose_layout(kj_ctx* c, const kj_index_view& v, uint32_t rep) {
+// With a host memory budget (kj_create_tiered, host_budget > 0), a compact index whose peak does not fit gets a host tier in mapped pinned host
+// memory instead, planned in this order, before anything large is allocated:
+//   tier 1: the suffix-array taxon and accession arrays (sa_tax, seq_tax, sa_acc, seq_acc; read once at the end of each SA walk) -- layout 2;
+//   tier 2: also the records [nb_dev, nb), nb_dev the largest count that leaves KJ_TIER_HEADROOM of HBM free -- layout 3 (compact tiered).
+// KJ_ERR_NOMEM when the host tier would exceed the budget.  KJ_TIER_DEVICE_RECORDS=n (developer hook, any compact index built with a budget):
+// nb_dev = n, tier 1 alone when n >= nb.
+static int kj_choose_layout(kj_ctx* c, const kj_index_view& v, uint32_t rep, uint64_t host_budget) {
     KjHostIndex& H = c->H;
     if (H.wide == KJ_LAYOUT_NARROW) return KJ_OK;
     const uint64_t n = H.bwtlen, alen = (uint64_t)H.alen;
@@ -293,12 +313,36 @@ static int kj_choose_layout(kj_ctx* c, const kj_index_view& v, uint32_t rep) {
     const uint64_t nb_c = n / KJ_RANK_ROWS_COMPACT + 1, nsb = kj_csb_count(n);
     const uint64_t compact_peak = peak(kj_rank_array_words(KJ_LAYOUT_COMPACT, H.alen, nb_c) * 8 + kj_letters_words(KJ_LAYOUT_COMPACT, n) * 8,
                                        nsb * KJ_CSB_STRIDE * 4 + (rep == 1 ? std::min(kj_compact_chunk_rows(), n) : (uint64_t)v.bwtlen));
-    if (compact_peak > fr) {
-        char b[256]; snprintf(b, sizeof b, "index of %llu rows does not fit in HBM: building it needs %llu bytes (compact layout), %llu bytes are free",
-                              (unsigned long long)n, (unsigned long long)compact_peak, (unsigned long long)fr);
+    const char* hook = host_budget ? getenv("KJ_TIER_DEVICE_RECORDS") : nullptr;
+    if (compact_peak <= fr && !hook) { H.wide = KJ_LAYOUT_COMPACT; H.nb = nb_c; c->nb_dev = nb_c; return KJ_OK; }
+    char b[400];
+    if (!host_budget) {
+        snprintf(b, sizeof b, "index of %llu rows does not fit in HBM: building it needs %llu bytes (compact layout), %llu bytes are free",
+                 (unsigned long long)n, (unsigned long long)compact_peak, (unsigned long long)fr);
         kj_err() = b; return KJ_ERR_NOMEM;
     }
-    H.wide = KJ_LAYOUT_COMPACT; H.nb = nb_c;
+    // the host tier: what stays in HBM is the superblock table, records [0, nd) and the largest transient buffer of the construction
+    const uint64_t rec = KJ_RANK_WORDS_COMPACT * 8, csb = kj_letters_words(KJ_LAYOUT_COMPACT, n) * 8;
+    const uint64_t transient = std::max(std::max(nsb * KJ_CSB_STRIDE * 4 + (rep == 1 ? std::min(kj_compact_chunk_rows(), n) : (uint64_t)v.bwtlen), upload), levels);
+    uint64_t nd = nb_c;
+    if (hook) nd = std::min<uint64_t>((uint64_t)std::max(0ll, atoll(hook)), nb_c);
+    else if (nb_c * rec + csb + transient + KJ_TIER_HEADROOM > fr) {
+        const uint64_t fixed = csb + transient + KJ_TIER_HEADROOM;
+        if (fixed > fr) {
+            snprintf(b, sizeof b, "index of %llu rows does not fit: %llu bytes of HBM are free, its superblock table and construction buffers need %llu bytes next to %llu bytes of headroom",
+                     (unsigned long long)n, (unsigned long long)fr, (unsigned long long)(csb + transient), (unsigned long long)KJ_TIER_HEADROOM);
+            kj_err() = b; return KJ_ERR_NOMEM;
+        }
+        nd = std::min<uint64_t>(nb_c, (fr - fixed) / rec);
+    }
+    const uint64_t host_need = sa + 64 + (nb_c - nd) * rec;
+    if (host_need > host_budget) {
+        snprintf(b, sizeof b, "index of %llu rows does not fit: %llu bytes of HBM are free, its host tier needs %llu bytes of pinned host memory, the budget (host_bytes) is %llu bytes",
+                 (unsigned long long)n, (unsigned long long)fr, (unsigned long long)host_need, (unsigned long long)host_budget);
+        kj_err() = b; return KJ_ERR_NOMEM;
+    }
+    H.wide = nd < nb_c ? KJ_LAYOUT_COMPACT_TIERED : KJ_LAYOUT_COMPACT; H.nb = nb_c; c->nb_dev = nd;
+    c->sa_tax.on_host = c->seq_tax.on_host = c->sa_acc.on_host = c->seq_acc.on_host = true;
     return KJ_OK;
 }
 
@@ -354,24 +398,16 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
     KjHostIndex& H = c->H; const uint64_t n = H.bwtlen; int rc;
     KjBuildLcode lc; memcpy(lc.v, lcode, 256);
     const int grid_big = c->sm_count * 16;
-    if ((rc = H.wide == KJ_LAYOUT_COMPACT ? kj_device_build_compact(c, v, lc, rep, tot) : kj_device_build_onehot(c, v, lc, rep, tot))) return rc;
-    // ---- sequence -> taxon, sampled suffix array -> taxon
-    if ((rc = upload(H.seq_tax, c->seq_tax, tot))) return rc;
-    if (!H.seq_acc.empty()) {
-        if ((rc = c->seq_acc.grow(H.seq_acc.size() * 4))) return rc;
-        tot += H.seq_acc.size() * 4; CK(cudaMemcpy(c->seq_acc.p, H.seq_acc.data(), H.seq_acc.size() * 4, cudaMemcpyHostToDevice));
-    }
+    if ((rc = kj_is_compact(H.wide) ? kj_device_build_compact(c, v, lc, rep, tot) : kj_device_build_onehot(c, v, lc, rep, tot))) return rc;
+    // ---- sequence -> taxon, sampled suffix array -> taxon (in HBM, or in the host tier: kj_choose_layout)
+    if ((rc = tier_upload(c, H.seq_tax, c->seq_tax, tot))) return rc;
+    if (!H.seq_acc.empty() && (rc = tier_upload(c, H.seq_acc, c->seq_acc, tot))) return rc;
     uint32_t* d_err = c->err.as<uint32_t>();
     uint64_t n_sa;
     if (rep == 1) {
         n_sa = (uint64_t)v.ncheck;
-        if ((rc = c->sa_tax.grow((n_sa + 1) * 4))) return rc;
-        tot += (n_sa + 1) * 4;
-        CK(cudaMemset(c->sa_tax.as<uint32_t>() + n_sa, 0xff, 4));       // guard entry (see create_ctx): the last sampled row has no entry in a reference-built index
-        if (c->seq_acc.p) {
-            if ((rc = c->sa_acc.grow((n_sa + 1) * 4))) return rc;
-            tot += (n_sa + 1) * 4; CK(cudaMemset(c->sa_acc.as<uint32_t>() + n_sa, 0xff, 4));
-        }
+        if ((rc = tier_grow(c, c->sa_tax, (n_sa + 1) * 4, tot)) || (rc = c->sa_tax.fill(n_sa * 4, 0xff, 4))) return rc;   // guard entry (see create_ctx): the last sampled row has no entry in a reference-built index
+        if (c->seq_acc.p && ((rc = tier_grow(c, c->sa_acc, (n_sa + 1) * 4, tot)) || (rc = c->sa_acc.fill(n_sa * 4, 0xff, 4)))) return rc;
         const uint64_t CHE = (uint64_t)1 << 26;                        // entries per upload chunk
         KjDevBuf sa; if ((rc = sa.grow((size_t)std::min<uint64_t>(CHE, std::max<uint64_t>(n_sa, 1)) * (size_t)v.nbytes))) return rc;
         for (uint64_t e0 = 0; e0 < n_sa; e0 += CHE) {
@@ -386,9 +422,9 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
     } else {
         const int64_t last = (int64_t)((n - 1) >> H.sa_exp) - H.sa_bias;  // entry of the last sampled row
         n_sa = last >= 0 ? (uint64_t)last + 1 : 0;
-        if ((rc = c->sa_tax.grow(std::max<size_t>(n_sa * 4, 16)))) return rc;
-        tot += std::max<size_t>(n_sa * 4, 16);
-        if (base->H.wide == KJ_LAYOUT_COMPACT) kj_bld_sa_tax_scaled<KjCompactIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        if ((rc = tier_grow(c, c->sa_tax, std::max<size_t>(n_sa * 4, 16), tot))) return rc;
+        if (base->H.wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_sa_tax_scaled<KjTieredIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        else if (base->H.wide == KJ_LAYOUT_COMPACT) kj_bld_sa_tax_scaled<KjCompactIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else kj_bld_sa_tax_scaled<uint32_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         CK(cudaGetLastError()); CK(cudaDeviceSynchronize()); c->launches++;
@@ -402,7 +438,8 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
 static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, int& k_out) {
     KjHostIndex& H = c->H; const int wide = H.wide; const KjDevIndex* ix = c->ix.as<KjDevIndex>();
     if (H.quirk_lo != ~0ull && &dst == &c->kmer) {
-        if (wide == KJ_LAYOUT_COMPACT) kj_bld_quirk<KjCompactIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_quirk<KjTieredIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        else if (wide == KJ_LAYOUT_COMPACT) kj_bld_quirk<KjCompactIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         else if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>()); else kj_bld_quirk<uint32_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         CK(cudaGetLastError()); CK(cudaMemcpy(H.quirk_d, c->quirk.p, sizeof H.quirk_d, cudaMemcpyDeviceToHost)); c->launches++;
     }
@@ -418,7 +455,8 @@ static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, 
     uint64_t n_cur = 20;
     for (int d = 1; d < k; d++) {
         const unsigned g = (unsigned)std::min<uint64_t>((n_cur * 20 + 255) / 256, (uint64_t)c->sm_count * 32);
-        if (wide == KJ_LAYOUT_COMPACT) kj_bld_kmer_level<KjCompactIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_kmer_level<KjTieredIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        else if (wide == KJ_LAYOUT_COMPACT) kj_bld_kmer_level<KjCompactIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         else if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>()); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         CK(cudaGetLastError()); c->launches++;
         std::swap(a, b); n_cur *= 20;

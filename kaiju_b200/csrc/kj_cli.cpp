@@ -21,6 +21,7 @@
 #include "kaiju_b200.h"
 
 static uint32_t g_max_read_len = KJ_MAX_READ_LEN;      // -L: longest mate admitted (kj_set_max_read_len)
+static uint64_t g_host_bytes = 0;                      // -H: pinned host memory the index may take when it does not fit in HBM (kj_create_tiered)
 static void die(const std::string& m);
 
 // ---- the name-reporting front-ends kaijux / kaijup (src/kaijux.cpp, kaijup.cpp, ConsumerThreadx.cpp:193-256, ConsumerThreadp.cpp:6-94) ----
@@ -76,7 +77,7 @@ int run_name_frontend(bool protein, kj_params P, const std::string& fmi_fn, cons
     iv.seq_taxon = st.data();
     kj_taxonomy_view tv; tv.n = node.size(); tv.node = node.data(); tv.parent = parent.data();
     P.name_mode = 1; P.input_is_protein = protein ? 1 : 0;
-    kj_ctx* ctx = nullptr; if (kj_create(&ctx, device, &P, &iv, &tv) != KJ_OK || kj_set_max_read_len(ctx, g_max_read_len) != KJ_OK) die(kj_last_error());
+    kj_ctx* ctx = nullptr; if (kj_create_tiered(&ctx, device, &P, &iv, &tv, 1, g_host_bytes) != KJ_OK || kj_set_max_read_len(ctx, g_max_read_len) != KJ_OK) die(kj_last_error());
     LineReader r1, r2; const bool paired = !in2.empty();
     if (!r1.open(in1)) die("Could not open file " + in1);
     if (paired && !r2.open(in2)) die("Could not open file " + in2);
@@ -166,14 +167,14 @@ static void usage(const char* prog) {
                     "   -z INT        accepted for compatibility (ignored: the GPU replaces the worker threads)\n   -a STRING     Run mode, either \"mem\"  or \"greedy\" (default: greedy)\n"
                     "   -e INT        Number of mismatches allowed in Greedy mode (default: 3)\n   -m INT        Minimum match length (default: 11)\n   -s INT        Minimum match score in Greedy mode (default: 65)\n"
                     "   -E FLOAT      Minimum E-value in Greedy mode (default: 0.01)\n   -x            Enable SEG low complexity filter (enabled by default)\n   -X            Disable SEG low complexity filter\n"
-                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  With several devices the data sets of the\n                 -i/-j/-o lists are classified in parallel, one context (index replica) per device\n", prog);
+                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -H GB         Pinned host memory (GiB) the index may take when it does not fit in GPU memory (default 0: GPU memory only); the part\n                 in host memory is read over PCIe, the results are the same\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  With several devices the data sets of the\n                 -i/-j/-o lists are classified in parallel, one context (index replica) per device\n", prog);
     exit(EXIT_FAILURE);
 }
 
 int main(int argc, char** argv) {
     kj_params P; P.mode = 1; P.min_fragment_length = 11; P.mismatches = 3; P.min_score = 65; P.seed_length = 7; P.use_evalue = 1; P.min_evalue = 0.01; P.seg = 1; P.input_is_protein = 0; P.name_mode = 0;
     std::string nodes_fn, fmi_fn, in1, in2, out_fn, native_out, table_fn, table_rank = "species", names_fn; bool verbose = false; std::string device_arg = "0", frontend; int c;
-    while ((c = getopt(argc, argv, "a:hd:pxXvn:m:e:E:l:t:f:i:j:s:z:o:w:T:r:N:M:L:")) != -1) {
+    while ((c = getopt(argc, argv, "a:hd:pxXvn:m:e:E:l:t:f:i:j:s:z:o:w:T:r:N:M:L:H:")) != -1) {
         switch (c) {
             case 'a': if (!strcmp(optarg, "mem")) { P.mode = 0; P.use_evalue = 0; } else if (!strcmp(optarg, "greedy")) P.mode = 1; else { fprintf(stderr, "-a must be a valid mode.\n"); usage(argv[0]); } break;
             case 'h': usage(argv[0]); break;
@@ -199,6 +200,7 @@ int main(int argc, char** argv) {
             case 'z': { if (atoi(optarg) <= 0) die("Number of threads (-z) must be greater than 0."); break; }
             case 'n': break;
             case 'M': frontend = optarg; break;
+            case 'H': { const double gb = atof(optarg); if (!(gb >= 0.0) || gb > 1e6) die("The host memory budget (-H) must be a number of GB >= 0."); g_host_bytes = (uint64_t)(gb * 1073741824.0); break; }
             case 'L': { const long v = atol(optarg); if (v < KJ_MAX_READ_LEN || v > KJ_MAX_LONG_READ_LEN) die("The read-length limit (-L) must lie between 16383 and 1048575."); g_max_read_len = (uint32_t)v; break; }
             default: usage(argv[0]);
         }
@@ -253,7 +255,7 @@ int main(int argc, char** argv) {
     {
         std::vector<std::thread> th; std::mutex mu; std::string err;
         for (size_t d = 0; d < devices.size(); d++) th.emplace_back([&, d] {
-            int rc = native_in ? kj_create_from_native(&ctxs[d], devices[d], &P, fmi_fn.c_str()) : kj_create(&ctxs[d], devices[d], &P, &iv, &tv);
+            int rc = native_in ? kj_create_from_native(&ctxs[d], devices[d], &P, fmi_fn.c_str()) : kj_create_tiered(&ctxs[d], devices[d], &P, &iv, &tv, 1, g_host_bytes);
             if (rc == KJ_OK) rc = kj_set_max_read_len(ctxs[d], g_max_read_len);
             if (rc != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); }
         });

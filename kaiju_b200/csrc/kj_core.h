@@ -148,6 +148,19 @@ typedef unsigned long long KjCompactIdx;
 template <class IdxT> struct KjIsCompact { static constexpr bool v = false; };
 template <> struct KjIsCompact<KjCompactIdx> { static constexpr bool v = true; };
 static_assert(sizeof(KjCompactIdx) == 8 && !KjIsCompact<uint64_t>::v, "KjCompactIdx must be a 64-bit type distinct from uint64_t");
+// The compact tiered layout (records [nb_dev, nb) in mapped host memory) runs them with IdxT = KjTieredIdx: a third 64-bit type, a row index
+// that converts to and from unsigned 64-bit integers, so the interval arithmetic of the kernels is that of the compact instantiation.
+struct KjTieredIdx {
+    unsigned long long v;
+    KjTieredIdx() = default;
+    KJ_HD constexpr KjTieredIdx(unsigned long long x) : v(x) {}
+    KJ_HD constexpr operator unsigned long long() const { return v; }
+    KJ_HD KjTieredIdx& operator-=(KjTieredIdx d) { v -= d.v; return *this; }
+};
+template <class IdxT> struct KjIsTiered { static constexpr bool v = false; };
+template <> struct KjIsTiered<KjTieredIdx> { static constexpr bool v = true; };
+static_assert(sizeof(KjTieredIdx) == 8 && !KjIsTiered<uint64_t>::v && !KjIsTiered<KjCompactIdx>::v && !KjIsCompact<KjTieredIdx>::v,
+              "KjTieredIdx must be a 64-bit type distinct from uint64_t and KjCompactIdx");
 // compact layout: rank of letter c at row k from the plane words of k's half-record `pl` (5 independent loads, issued by the caller) plus the
 // midpoint count and the superblock count -- every address a function of (c, k) only, and no branch on the data
 static KJ_DEV uint64_t kj_crank_planes(const KjDevIndex& ix, const uint64_t* rec, const uint64_t pw[5], uint32_t c, uint64_t k) {
@@ -163,19 +176,30 @@ static KJ_DEV uint64_t kj_crank_planes(const KjDevIndex& ix, const uint64_t* rec
     const uint64_t v = sb + ((cw >> (16u * (c & 3u))) & 0xffffull);
     return h ? v + pc : v - pc;
 }
-static KJ_DEV const uint64_t* kj_crec(const KjDevIndex& ix, uint64_t k) { return ix.rank + (size_t)(k >> 7) * KJ_RANK_WORDS_COMPACT; }
+// TIER = true (compact tiered layout): the record lies in HBM below the split, in mapped host memory above it -- the base and the index are
+// selected, not branched on, so the load addresses still follow from (c, k) alone
+template <bool TIER = false>
+static KJ_DEV const uint64_t* kj_crec(const KjDevIndex& ix, uint64_t k) {
+    if constexpr (TIER) {
+        const uint64_t b = k >> 7, nd = ix.tier.nb_dev; const bool dev = b < nd;
+        const uint64_t* base = dev ? ix.rank : ix.tier.host;
+        return base + (size_t)(dev ? b : b - nd) * KJ_RANK_WORDS_COMPACT;
+    } else return ix.rank + (size_t)(k >> 7) * KJ_RANK_WORDS_COMPACT;
+}
 static KJ_DEV void kj_cplanes(const uint64_t* rec, uint64_t k, uint64_t pw[5]) {
     const uint64_t* pl = rec + 5u * ((uint32_t)(k >> 6) & 1u);
     #pragma unroll
     for (int b = 0; b < 5; b++) pw[b] = kj_ld64(pl + b);
 }
+template <bool TIER = false>
 static KJ_DEV uint64_t kj_crank(const KjDevIndex& ix, uint32_t c, uint64_t k) {
-    const uint64_t* rec = kj_crec(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    const uint64_t* rec = kj_crec<TIER>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
     return kj_crank_planes(ix, rec, pw, c, k);
 }
 // one LF step of the compact layout: the letter of row k and its rank, from k's record
+template <bool TIER = false>
 static KJ_DEV uint64_t kj_clf(const KjDevIndex& ix, uint64_t k, uint32_t& c) {
-    const uint64_t* rec = kj_crec(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    const uint64_t* rec = kj_crec<TIER>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
     const uint32_t bit = (uint32_t)k & 63u; c = 0;
     #pragma unroll
     for (int b = 0; b < 5; b++) c |= (uint32_t)((pw[b] >> bit) & 1ull) << b;
@@ -185,6 +209,7 @@ static KJ_DEV const uint64_t* kj_letter_base(const KjDevIndex& ix, uint32_t c) {
 template <class IdxT>
 static KJ_DEV IdxT kj_rank(const KjDevIndex& ix, uint32_t c, IdxT k) {
     if constexpr (KjIsCompact<IdxT>::v) return (IdxT)kj_crank(ix, c, (uint64_t)k);
+    else if constexpr (KjIsTiered<IdxT>::v) return (IdxT)kj_crank<true>(ix, c, (uint64_t)k);
     else return kj_rank_at<IdxT>(kj_letter_base(ix, c), k);
 }
 // UpdateSI (bwt.c:160-173)
@@ -192,6 +217,7 @@ template <class IdxT>
 static KJ_DEV bool kj_update_si(const KjDevIndex& ix, uint32_t c, IdxT& lo, IdxT& hi) {
     IdxT nlo, nhi;
     if constexpr (KjIsCompact<IdxT>::v) { nlo = (IdxT)kj_crank(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank(ix, c, (uint64_t)hi); }
+    else if constexpr (KjIsTiered<IdxT>::v) { nlo = (IdxT)kj_crank<true>(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank<true>(ix, c, (uint64_t)hi); }
     else { const uint64_t* base = kj_letter_base(ix, c); nlo = kj_rank_at<IdxT>(base, lo); nhi = kj_rank_at<IdxT>(base, hi); }
     // the reference's checkpoint quirk (indexes with bwtlen = m * 2^16 only, kj_host.cpp): the last 129 positions rank lower by a per-letter
     // constant.  Such indexes are routed to the 64-bit kernels, so the 32-bit ones do not carry the test.
@@ -221,6 +247,7 @@ static KJ_DEV uint64_t kj_sa_locate(const KjDevIndex& ix, uint64_t k, bool& is_s
     KJ_ROLLED
     while (c != 0 && (k & ix.sa_check)) {
         if constexpr (KjIsCompact<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf(ix, k, c); if (q) k -= ix.quirk_d[c]; }
+        else if constexpr (KjIsTiered<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf<true>(ix, k, c); if (q) k -= ix.quirk_d[c]; }
         else { c = kj_letter(ix, k); const bool q = k >= ix.quirk_lo; k = (uint64_t)kj_rank<IdxT>(ix, c, (IdxT)k); if (q) k -= ix.quirk_d[c]; }
 #if defined(KJ_EMU)
         kj_emu_stats.sa_lf_steps++;

@@ -171,14 +171,16 @@ static KjKernel kj_select_kernel_t(bool gws, bool fixed, bool verbose, int role)
 }
 template <int MODE, class T>
 static KjKernel kj_select_long_kernel_t(bool verbose) { return verbose ? kj_classify_long_kernel<MODE, T, true> : kj_classify_long_kernel<MODE, T, false>; }
-// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact (64-bit intervals; kj_layout.h).  long_reads: the batch holds mates longer than
+// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact, 3 compact tiered (64-bit intervals; kj_layout.h).  long_reads: the batch holds mates longer than
 // KJ_MAX_READ_LEN (only the work space in global memory, the general profile and ROLE 0 exist for them).
 static KjKernel kj_select_kernel(int mode, int layout, bool gws, bool fixed, bool verbose, int role, bool long_reads = false) {
     if (long_reads) {
+        if (layout == KJ_LAYOUT_COMPACT_TIERED) return mode == 0 ? kj_select_long_kernel_t<0, KjTieredIdx>(verbose) : kj_select_long_kernel_t<1, KjTieredIdx>(verbose);
         if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_long_kernel_t<0, KjCompactIdx>(verbose) : kj_select_long_kernel_t<1, KjCompactIdx>(verbose);
         if (mode == 0) return layout ? kj_select_long_kernel_t<0, uint64_t>(verbose) : kj_select_long_kernel_t<0, uint32_t>(verbose);
         return layout ? kj_select_long_kernel_t<1, uint64_t>(verbose) : kj_select_long_kernel_t<1, uint32_t>(verbose);
     }
+    if (layout == KJ_LAYOUT_COMPACT_TIERED) return mode == 0 ? kj_select_kernel_t<0, KjTieredIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjTieredIdx>(gws, fixed, verbose, role);
     if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_kernel_t<0, KjCompactIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjCompactIdx>(gws, fixed, verbose, role);
     if (mode == 0) return layout ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
     return layout ? kj_select_kernel_t<1, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<1, uint32_t>(gws, fixed, verbose, role);
@@ -229,6 +231,35 @@ struct KjDevBuf {
     template <class T> T* as() const { return (T*)p; }
 };
 
+// The host-side counterpart of KjDevBuf: pinned host memory mapped into the device's address space (the host tier of kj_create_tiered).
+// `p` is the host address, `d` the device alias the kernels read it through.  Move-only, freed by its destructor.
+struct KjHostBuf {
+    void* p = nullptr; void* d = nullptr; size_t cap = 0;
+    KjHostBuf() = default;
+    KjHostBuf(const KjHostBuf&) = delete; KjHostBuf& operator=(const KjHostBuf&) = delete;
+    KjHostBuf(KjHostBuf&& o) noexcept : p(o.p), d(o.d), cap(o.cap) { o.p = o.d = nullptr; o.cap = 0; }
+    KjHostBuf& operator=(KjHostBuf&& o) noexcept { if (this != &o) { reset(); p = o.p; d = o.d; cap = o.cap; o.p = o.d = nullptr; o.cap = 0; } return *this; }
+    ~KjHostBuf() { reset(); }
+    void reset() { if (p) cudaFreeHost(p); p = d = nullptr; cap = 0; }
+    int grow(size_t need) {
+        if (need <= cap) return KJ_OK;
+        reset(); void* q = nullptr; CK(cudaHostAlloc(&q, need, cudaHostAllocMapped)); p = q; cap = need;
+        void* dq = nullptr; CK(cudaHostGetDevicePointer(&dq, q, 0)); d = dq; return KJ_OK;
+    }
+    template <class T> T* as() const { return (T*)d; }
+};
+// An index array the placement of kj_create_tiered may move to the host tier (kj_choose_layout sets on_host before it is allocated): in HBM or
+// in mapped pinned host memory, read by the kernels through `p` either way.
+struct KjTierBuf {
+    KjDevBuf dev; KjHostBuf host; bool on_host = false; void* p = nullptr;
+    int grow(size_t need) { const int rc = on_host ? host.grow(need) : dev.grow(need); p = on_host ? host.d : dev.p; return rc; }
+    template <class T> T* as() const { return (T*)p; }
+    size_t cap() const { return on_host ? host.cap : dev.cap; }
+    // bytes [off, off + n) = val; the host tier is written by the CPU (nothing on the device writes it at this point)
+    int fill(size_t off, int val, size_t n) { if (on_host) memset((char*)host.p + off, val, n); else CK(cudaMemset((char*)dev.p + off, val, n)); return KJ_OK; }
+    int put(const void* src, size_t n) { if (on_host) memcpy(host.p, src, n); else CK(cudaMemcpy(dev.p, src, n, cudaMemcpyHostToDevice)); return KJ_OK; }
+};
+
 // One of the two pipeline slots (the chunks of kj_classify, the lanes of kj_classify_files): staging, outputs, scratch, streams.
 // Two slots may be in flight, and their launches may have different run parameters (kj_classify_files derives them from each batch's longest
 // read): each slot has its own scratch, sized and grown from that slot's launches alone.  Carving both slots out of one buffer at offsets
@@ -255,9 +286,11 @@ struct kj_ctx {
     KjDevIndex dix{};              // host copy of the descriptor (device pointers inside)
     KjDevBuf ix, tables;
     KjDevBuf ix_mem, kmer_mem; int kmer_k_mem = 0;      // the MEM kernels' own descriptor: same index, 7-mer table (kj_create)
-    KjDevBuf rank, letters, sa_tax, seq_tax, sa_acc, seq_acc, tax_parent, tax_depth, tax_id, lnfact, kmer;    // compact layout: `letters` holds the superblock table
+    KjDevBuf rank, letters, tax_parent, tax_depth, tax_id, lnfact, kmer;    // compact layout: `letters` holds the superblock table
+    KjTierBuf sa_tax, seq_tax, sa_acc, seq_acc;     // in HBM, or in the host tier of a kj_create_tiered context
+    KjHostBuf rank_host; uint64_t nb_dev = 0;       // compact tiered layout: records [nb_dev, nb) in the host tier, records [0, nb_dev) in `rank`
     KjDevBuf row_tax;              // taxon per BWT row (kj_device_build_row_tax; empty: the kernels walk)
-    uint64_t index_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;
+    uint64_t index_bytes = 0, host_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;      // HBM and pinned host memory of the index
     // run state
     KjDevBuf counter, err, maxlen, quirk;
     KjDevBuf evbreaks; uint32_t n_evbreaks = 0;
@@ -286,6 +319,15 @@ template <class T> static int upload(const std::vector<T>& v, KjDevBuf& d, uint6
     int rc = d.grow(bytes); if (rc) return rc;
     if (!v.empty()) CK(cudaMemcpy(d.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
     total += bytes; return KJ_OK;
+}
+// an array that may live in the host tier: its bytes count towards the context's host bytes there, towards `total` (HBM) otherwise
+static int tier_grow(kj_ctx* c, KjTierBuf& b, size_t bytes, uint64_t& total) {
+    int rc = b.grow(bytes); if (rc) return rc;
+    (b.on_host ? c->host_bytes : total) += bytes; return KJ_OK;
+}
+template <class T> static int tier_upload(kj_ctx* c, const std::vector<T>& v, KjTierBuf& b, uint64_t& total) {
+    int rc = tier_grow(c, b, std::max<size_t>(v.size() * sizeof(T), 16), total); if (rc) return rc;
+    return v.empty() ? KJ_OK : b.put(v.data(), v.size() * sizeof(T));
 }
 
 // Shared-memory work space while three CTAs still fit on an SM; beyond that (mates longer than ~280 bases) the same
@@ -351,7 +393,8 @@ static int upload_descriptor(kj_ctx* c) {
     KjHostIndex& H = c->H; KjDevIndex& D = c->dix; memset(&D, 0, sizeof D);
     D.rank = c->rank.as<const uint64_t>(); D.nb = H.nb; D.letters = c->letters.as<const uint64_t>(); D.bwtlen = H.bwtlen; D.alen = H.alen;
     for (int a = 0; a <= H.alen; a++) D.C[a] = H.C[a];
-    if (H.wide != KJ_LAYOUT_COMPACT) for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
+    if (!kj_is_compact(H.wide)) for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
+    if (H.wide == KJ_LAYOUT_COMPACT_TIERED) { D.tier.host = c->rank_host.as<const uint64_t>(); D.tier.nb_dev = c->nb_dev; }
     D.sa_acc = c->sa_acc.as<const uint32_t>(); D.seq_acc = c->seq_acc.as<const uint32_t>();
     D.sa_tax = c->sa_tax.as<const uint32_t>(); D.seq_tax = c->seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
     D.n_sa = c->n_sa; D.row_tax = c->row_tax.as<const uint32_t>(); D.nseq = H.nseq;
@@ -404,9 +447,9 @@ template <class Fill> static int create_ctx(kj_ctx** out, int device, const kj_p
     // one guard entry: the reference's header counts one sampled row less than kaiju-mkbwt writes (suffixArray.c:160 vs 206-216), so the last
     // sampled row of an index has no entry; the reference reads past its array there, the device reads "no taxon"
     c->n_sa = H.sa_tax.size(); H.sa_tax.push_back(KJ_TAX_BAD);
-    if (!H.seq_acc.empty()) { H.sa_acc.push_back(0xffffffffu); if ((rc = upload(H.sa_acc, c->sa_acc, tot)) || (rc = upload(H.seq_acc, c->seq_acc, tot))) return rc; }
-    if ((rc = upload(H.rank, c->rank, tot)) || (rc = upload(H.letters, c->letters, tot)) || (rc = upload(H.sa_tax, c->sa_tax, tot)) ||
-        (rc = upload(H.seq_tax, c->seq_tax, tot)) || (rc = upload_small(c, tot)) || (rc = (H.wide ? upload(H.kmer, c->kmer, tot) : upload(H.kmer32, c->kmer, tot)))) return rc;
+    if (!H.seq_acc.empty()) { H.sa_acc.push_back(0xffffffffu); if ((rc = tier_upload(c, H.sa_acc, c->sa_acc, tot)) || (rc = tier_upload(c, H.seq_acc, c->seq_acc, tot))) return rc; }
+    if ((rc = upload(H.rank, c->rank, tot)) || (rc = upload(H.letters, c->letters, tot)) || (rc = tier_upload(c, H.sa_tax, c->sa_tax, tot)) ||
+        (rc = tier_upload(c, H.seq_tax, c->seq_tax, tot)) || (rc = upload_small(c, tot)) || (rc = (H.wide ? upload(H.kmer, c->kmer, tot) : upload(H.kmer32, c->kmer, tot)))) return rc;
     // host copies of the big arrays are no longer needed
     std::vector<uint64_t>().swap(H.rank); std::vector<uint64_t>().swap(H.letters); std::vector<uint32_t>().swap(H.sa_tax); std::vector<KjKmer>().swap(H.kmer); std::vector<KjKmer32>().swap(H.kmer32);
     if ((rc = finish_ctx(c, tot))) return rc;
@@ -414,13 +457,15 @@ template <class Fill> static int create_ctx(kj_ctx** out, int device, const kj_p
 }
 
 #include "kj_build.h"
-// kj_create / kj_create_scaled: the large arrays are built on the device from the raw BWT bytes and suffix-array samples (kj_build.h)
-static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, const kj_index_view& v, const kj_taxonomy_view& t, uint32_t copies, const kj_ctx* base) {
+// kj_create / kj_create_scaled / kj_create_tiered: the large arrays are built on the device from the raw BWT bytes and suffix-array samples
+// (kj_build.h); host_budget > 0: a compact index that does not fit in HBM may take up to that many bytes of pinned host memory (kj_choose_layout)
+static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, const kj_index_view& v, const kj_taxonomy_view& t, uint32_t copies, const kj_ctx* base,
+                             uint64_t host_budget) {
     kj_ctx* c = nullptr; int rc = new_ctx(&c, device, params); if (rc) return rc;
     std::unique_ptr<kj_ctx, void (*)(kj_ctx*)> guard(c, kj_destroy);
     const auto t0 = std::chrono::steady_clock::now();
     uint8_t lcode[256]; rc = kj_build_host_meta(v, t, copies, c->H, lcode); if (rc) return rc;
-    if ((rc = kj_choose_layout(c, v, copies))) return rc;
+    if ((rc = kj_choose_layout(c, v, copies, host_budget))) return rc;
     uint64_t tot = 0;
     if ((rc = upload_small(c, tot)) || (rc = kj_device_build(c, v, lcode, copies, base, tot))) return rc;
     c->H.kmer_k = 0;
@@ -443,26 +488,42 @@ static int create_ctx_device(kj_ctx** out, int device, const kj_params* params, 
 extern "C" int kj_create(kj_ctx** out, int device, const kj_params* params, const kj_index_view* index, const kj_taxonomy_view* taxonomy) {
     if (!out || !params || !index || !taxonomy) { kj_err() = "kj_create: null argument"; return KJ_ERR_ARG; }
     if (getenv("KJ_HOST_BUILD")) return create_ctx(out, device, params, [&](KjHostIndex& H) { return kj_build_host_index(*index, *taxonomy, H); });   // developer hook: host transcoder + upload
-    return create_ctx_device(out, device, params, *index, *taxonomy, 1, nullptr);
+    return create_ctx_device(out, device, params, *index, *taxonomy, 1, nullptr, 0);
+}
+static int create_scaled(kj_ctx** out, int device, const kj_params* params, const kj_index_view* index, const kj_taxonomy_view* taxonomy, uint32_t copies, uint64_t host_budget) {
+    if (copies <= 1) return create_ctx_device(out, device, params, *index, *taxonomy, 1, nullptr, host_budget);
+    kj_ctx* base = nullptr; kj_transient_ctx = true; int rc = create_ctx_device(&base, device, params, *index, *taxonomy, 1, nullptr, host_budget); kj_transient_ctx = false; if (rc) return rc;
+    rc = create_ctx_device(out, device, params, *index, *taxonomy, copies, base, host_budget);
+    kj_destroy(base);
+    return rc;
 }
 extern "C" int kj_create_scaled(kj_ctx** out, int device, const kj_params* params, const kj_index_view* index, const kj_taxonomy_view* taxonomy, uint32_t copies) {
     if (!out || !params || !index || !taxonomy) { kj_err() = "kj_create_scaled: null argument"; return KJ_ERR_ARG; }
     if (copies <= 1) return kj_create(out, device, params, index, taxonomy);
-    kj_ctx* base = nullptr; kj_transient_ctx = true; int rc = create_ctx_device(&base, device, params, *index, *taxonomy, 1, nullptr); kj_transient_ctx = false; if (rc) return rc;
-    rc = create_ctx_device(out, device, params, *index, *taxonomy, copies, base);
-    kj_destroy(base);
-    return rc;
+    return create_scaled(out, device, params, index, taxonomy, copies, 0);
+}
+extern "C" int kj_create_tiered(kj_ctx** out, int device, const kj_params* params, const kj_index_view* index, const kj_taxonomy_view* taxonomy, uint32_t copies, uint64_t host_bytes) {
+    if (!out || !params || !index || !taxonomy) { kj_err() = "kj_create_tiered: null argument"; return KJ_ERR_ARG; }
+    if (host_bytes == 0) return kj_create_scaled(out, device, params, index, taxonomy, copies);
+    return create_scaled(out, device, params, index, taxonomy, copies < 1 ? 1 : copies, host_bytes);
 }
 extern "C" double kj_index_build_ms(const kj_ctx* c) { return c ? c->build_ms : 0.0; }
-// test hook: checksums of the index arrays as they sit in HBM (rank, letters or the compact superblock table, sa_tax, seq_tax, kmer | bwtlen,
-// layout, n_sa), to compare the device construction with the host transcoder array for array
+// test hook: checksums of the index arrays as they sit in memory (rank, letters or the compact superblock table, sa_tax, seq_tax, kmer | bwtlen,
+// layout, n_sa), to compare the device construction with the host transcoder array for array.  The records of a compact tiered index are its
+// HBM part followed by its host part.
 extern "C" int kj_debug_index_checksums(kj_ctx* c, uint64_t out[8]) {
     if (!c || !out) return KJ_ERR_ARG; CK(cudaSetDevice(c->device)); CK(cudaDeviceSynchronize());
     const KjHostIndex& H = c->H; memset(out, 0, 64);
     const size_t sz[5] = {(size_t)kj_rank_array_words(H.wide, H.alen, H.nb) * 8, (size_t)kj_letters_words(H.wide, H.bwtlen) * 8, (size_t)c->n_sa * 4, (size_t)H.nseq * 4,
                           H.kmer_k ? (size_t)pow(20.0, H.kmer_k) * (H.wide ? sizeof(KjKmer) : sizeof(KjKmer32)) : 0};
     const void* ptr[5] = {c->rank.p, c->letters.p, c->sa_tax.p, c->seq_tax.p, c->kmer.p};
-    for (int i = 0; i < 5; i++) { std::vector<uint8_t> h(sz[i]); if (sz[i]) CK(cudaMemcpy(h.data(), ptr[i], sz[i], cudaMemcpyDeviceToHost)); out[i] = kj_mix_bytes(0x6b616a75ull + i, h.data(), h.size()); }
+    const size_t dev0 = H.wide == KJ_LAYOUT_COMPACT_TIERED ? (size_t)c->nb_dev * KJ_RANK_WORDS_COMPACT * 8 : sz[0];      // bytes of the records in HBM
+    for (int i = 0; i < 5; i++) {
+        std::vector<uint8_t> h(sz[i]); const size_t nd = i == 0 ? dev0 : sz[i];
+        if (nd) CK(cudaMemcpy(h.data(), ptr[i], nd, cudaMemcpyDefault));
+        if (i == 0 && sz[0] > dev0) memcpy(h.data() + dev0, c->rank_host.p, sz[0] - dev0);
+        out[i] = kj_mix_bytes(0x6b616a75ull + i, h.data(), h.size());
+    }
     out[5] = H.bwtlen; out[6] = (uint64_t)H.wide; out[7] = c->n_sa;
     return KJ_OK;
 }
@@ -820,6 +881,7 @@ extern "C" int kj_classify_verbose2(kj_ctx* c, const char* seq1, const uint64_t*
 }
 extern "C" uint64_t kj_kernel_launches(const kj_ctx* c) { return c ? c->launches : 0; }
 extern "C" uint64_t kj_index_bytes(const kj_ctx* c) { return c ? c->index_bytes : 0; }
+extern "C" uint64_t kj_index_host_bytes(const kj_ctx* c) { return c ? c->host_bytes : 0; }
 extern "C" int kj_index_layout(const kj_ctx* c) { return c ? c->H.wide : -1; }
 extern "C" double kj_last_kernel_ms(const kj_ctx* c) {
     if (!c) return 0.0;

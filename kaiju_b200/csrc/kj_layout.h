@@ -19,6 +19,7 @@
 //   tax_*      : taxonomy re-indexed densely: ids present in nodes.dmp get indices [0,n_present), DB taxa
 //                absent from nodes.dmp get the indices after that (depth 0 marks "absent", util.cpp:206).
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 // Three record layouts, chosen per index at load time:
@@ -32,10 +33,14 @@
 //          per superblock).  FMindex(c,k) = csb + mid count +/- the popcount of "plane word == c" between k and the midpoint: 5 plane words, one
 //          count word and one superblock word, all addressed from (c,k) alone.  The same record gives the letter of row k (no `letters` array).
 //          1.003 B per row: refseq_ref (2.7e10 rows) fits an 80 GB H100.  Rows past bwtlen hold letter 31, which no rank query counts.
-// Layout codes (KjDevIndex::wide, KjHostIndex::wide): 0 narrow, 1 wide, 2 compact.
+//   compact tiered (kj_create_tiered, indexes whose compact construction does not fit in HBM either): the compact records, split at record
+//          nb_dev: records [0, nb_dev) in HBM, records [nb_dev, nb) in pinned host memory mapped into the device's address space (read over PCIe).
+//          Everything else of the index stays in HBM.  The record format is the compact one; only the address of record b depends on the split.
+// Layout codes (KjDevIndex::wide, KjHostIndex::wide): 0 narrow, 1 wide, 2 compact, 3 compact tiered.
 #define KJ_LAYOUT_NARROW 0
 #define KJ_LAYOUT_WIDE 1
 #define KJ_LAYOUT_COMPACT 2
+#define KJ_LAYOUT_COMPACT_TIERED 3
 #define KJ_RANK_ROWS_NARROW 64
 #define KJ_RANK_ROWS_WIDE 192
 #define KJ_RANK_ROWS_COMPACT 128
@@ -45,14 +50,15 @@
 #define KJ_CPT_COUNT_WORD 10       // compact record: the 16-bit midpoint counts start at word 10
 #define KJ_CSB_SHIFT 16            // compact superblock: 2^16 rows = 512 records
 #define KJ_CSB_STRIDE 24           // compact superblock table: words per superblock (KJ_MAX_ALEN)
-static inline uint32_t kj_rank_rows(int layout) { return layout == KJ_LAYOUT_COMPACT ? KJ_RANK_ROWS_COMPACT : layout ? KJ_RANK_ROWS_WIDE : KJ_RANK_ROWS_NARROW; }
-static inline uint32_t kj_rank_words(int layout) { return layout == KJ_LAYOUT_COMPACT ? KJ_RANK_WORDS_COMPACT : layout ? KJ_RANK_WORDS_WIDE : KJ_RANK_WORDS_NARROW; }
+static inline bool kj_is_compact(int layout) { return layout == KJ_LAYOUT_COMPACT || layout == KJ_LAYOUT_COMPACT_TIERED; }     // the compact record format
+static inline uint32_t kj_rank_rows(int layout) { return kj_is_compact(layout) ? KJ_RANK_ROWS_COMPACT : layout ? KJ_RANK_ROWS_WIDE : KJ_RANK_ROWS_NARROW; }
+static inline uint32_t kj_rank_words(int layout) { return kj_is_compact(layout) ? KJ_RANK_WORDS_COMPACT : layout ? KJ_RANK_WORDS_WIDE : KJ_RANK_WORDS_NARROW; }
 // 64-bit words of the rank array: one record per (letter, block) in the one-hot layouts, one record per block in the compact one
-static inline uint64_t kj_rank_array_words(int layout, int alen, uint64_t nb) { return (layout == KJ_LAYOUT_COMPACT ? 1ull : (uint64_t)alen) * nb * kj_rank_words(layout); }
+static inline uint64_t kj_rank_array_words(int layout, int alen, uint64_t nb) { return (kj_is_compact(layout) ? 1ull : (uint64_t)alen) * nb * kj_rank_words(layout); }
 static inline uint64_t kj_csb_count(uint64_t bwtlen) { return (bwtlen >> KJ_CSB_SHIFT) + 1; }     // superblocks of a compact index (k = bwtlen included)
 #define KJ_LETTERS_PER_WORD 12
 // 64-bit words of the `letters` array: the packed letters, or the superblock table of the compact layout
-static inline uint64_t kj_letters_words(int layout, uint64_t bwtlen) { return layout == KJ_LAYOUT_COMPACT ? kj_csb_count(bwtlen) * KJ_CSB_STRIDE : bwtlen / KJ_LETTERS_PER_WORD + 2; }
+static inline uint64_t kj_letters_words(int layout, uint64_t bwtlen) { return kj_is_compact(layout) ? kj_csb_count(bwtlen) * KJ_CSB_STRIDE : bwtlen / KJ_LETTERS_PER_WORD + 2; }
 #define KJ_MAX_ALEN 24
 #define KJ_MAX_IDS 21              // max_match_ids = 20 -> the set holds at most 21 (ConsumerThread.cpp:805)
 #define KJ_MAX_BEST_SI 20          // max_matches_SI (Config.hpp:35)
@@ -79,10 +85,16 @@ struct KjTables {
     uint8_t aa_index[32];            // protein input: upper-case letter - 'A' -> alphabet index, 0 = splits the read (ConsumerThread.cpp:664)
 };
 
+// compact tiered layout: records [nb_dev, nb) start at `host` (the device alias of mapped pinned host memory), record b at host + (b - nb_dev) * 16
+struct KjTierRef { const uint64_t* host; uint64_t nb_dev; };
 // (the 32-bit members are paired so that the descriptor has no padding holes: the kernels stage it in shared memory next to the work spaces)
 struct KjDevIndex {
     const uint64_t* rank; uint64_t nb;          // [alen][nb] records of 2 (narrow) or 4 (wide) 64-bit words; compact: [nb] records of 16 words
-    const uint64_t* rank_base[KJ_MAX_ALEN];     // records of letter c (saves the multiply in the inner loop; not used by the compact layout)
+                                                // (compact tiered: records [0, tier.nb_dev) only)
+    union {
+        const uint64_t* rank_base[KJ_MAX_ALEN]; // narrow, wide: records of letter c (saves the multiply in the inner loop)
+        KjTierRef tier;                         // compact tiered: where records [nb_dev, nb) are (the compact layouts do not use rank_base)
+    };
     union {
         const uint64_t* letters;                // narrow, wide: the packed letters
         const uint64_t* csb;                    // compact: [superblock][KJ_CSB_STRIDE] C[c] + #c before the superblock
@@ -96,11 +108,15 @@ struct KjDevIndex {
     const uint32_t* tax_parent; const uint32_t* tax_depth; const uint64_t* tax_id; uint32_t n_tax; int n_lnfact;
     const double* lnfact;
     const void* kmer; int kmer_k;               // direct-address table of k-mer intervals (KjKmer32 if !wide else KjKmer; 0 = off)
-    int wide;                                   // layout code: 0 narrow (32-bit interval kernels), 1 wide, 2 compact (64-bit interval kernels)
+    int wide;                                   // layout code: 0 narrow (32-bit interval kernels), 1 wide, 2 compact, 3 compact tiered (64-bit interval kernels)
     int mono;                                   // 1: true FM index (match starts monotone in the end position); 0: the reference's checkpoint quirk applies (no chain bounds)
     uint64_t quirk_lo; const uint64_t* quirk_d;         // rows k >= quirk_lo: FMindex(c,k) -= quirk_d[c] (reference checkpoint quirk, ~0 = none; [KJ_MAX_ALEN] in global memory)
     const KjTables* tables;
 };
+// The tier reference shares rank_base's bytes: the descriptor keeps the size and member offsets the shared-memory carve-up and the launch
+// geometry of every kernel were derived from.
+static_assert(sizeof(KjTierRef) <= sizeof(const uint64_t*) * KJ_MAX_ALEN && sizeof(KjDevIndex) == 592 && offsetof(KjDevIndex, rank_base) == 16 &&
+              offsetof(KjDevIndex, tier) == 16 && offsetof(KjDevIndex, letters) == 208 && offsetof(KjDevIndex, tables) == 584, "KjDevIndex layout changed");
 
 struct KjRunParams {
     int mode;                       // 0 MEM, 1 GREEDY
