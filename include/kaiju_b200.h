@@ -192,9 +192,15 @@ int kj_device_count(void);                        /* number of usable CUDA devic
  * lines "C\t<name>\t<taxid>" / "U\t<name>\t0" (verbose: plus "\t<best>\t<id,id,...,>") are formatted on the device and
  * written to out_path (NULL or "" = stdout) in INPUT order.  FASTQ = 4-line records; empty lines before the first and between
  * records are skipped as the reference's reader does (kaiju.cpp:288-289, 341-348).  Errors mirror the
- * reference's messages (file type detection, differing read names, file 1 longer than file 2) as KJ_ERR_IO. */
+ * reference's messages (file type detection, differing read names, file 1 longer than file 2) as KJ_ERR_IO.
+ * gzip input: a blocked gzip file (BGZF, what `bgzip` writes: the first member carries the "BC" extra subfield) is inflated on the device, one
+ * block per warp, CRC-32 and length of every block checked there; only the compressed bytes cross to the device.  Should a later member of
+ * such a file not be a BGZF block, zlib reads the rest from there.  Every other gzip file is inflated by zlib on one host thread per file.
+ * A corrupt or truncated BGZF block is KJ_ERR_IO, and kj_last_error() names the file and the block's offset in it. */
 int kj_classify_files(kj_ctx *ctx, const char *in1, const char *in2, const char *out_path, int verbose,
                       uint64_t *n_reads_out, uint64_t *n_classified_out);
+/* Bytes of text the device inflated in the last kj_classify_files call of the context (both input files; 0 for plain and zlib input). */
+uint64_t kj_files_device_inflated_bytes(const kj_ctx *ctx);
 
 /* --- per-taxon read counts (SURVEY.md 8f-3: what kaiju2table's first pass computes, src/kaiju2table.cpp:186-245) --- */
 /* Every successful kj_classify / kj_classify_verbose / kj_classify_files call adds its reads to a dense count vector in HBM:
@@ -243,7 +249,7 @@ uint64_t kj_index_host_bytes(const kj_ctx *ctx);  /* bytes of pinned host memory
  * fits, kj_create / kj_create_scaled fail with KJ_ERR_NOMEM and kj_last_error() names the bytes needed and the bytes free (kj_create_tiered:
  * see there).  -1 for a null context. */
 int kj_index_layout(const kj_ctx *ctx);
-double kj_last_kernel_ms(const kj_ctx *ctx);      /* device time of the last classify kernel (CUDA events) */
+double kj_last_kernel_ms(const kj_ctx *ctx);      /* device time of the last classify kernel, or of kj_debug_inflate_bgzf's kernel (CUDA events) */
 int kj_launch_geometry(const kj_ctx *ctx, int *grid, int *block, int *dyn_smem_bytes);  /* of the last classify launch */
 int kj_version(void);
 /* test hooks: checksums of the index arrays (rank, letters, sa_tax, seq_tax, kmer | bwtlen, layout, n_sa) as held in HBM by a context (compact
@@ -251,6 +257,11 @@ int kj_version(void);
  * and the same from the host transcoder (no GPU needed) -- the device construction is tested against the host one array for array */
 int kj_debug_index_checksums(kj_ctx *ctx, uint64_t out[8]);
 int kj_debug_host_index_checksums(const kj_index_view *index, const kj_taxonomy_view *taxonomy, uint64_t out[8]);
+/* test hook: a whole BGZF file held in host memory through the header walk and the inflate kernel of kj_classify_files; the text goes to
+ * out[0, *out_n).  KJ_ERR_IO and the compressed offset of the first bad block in *first_bad_offset for a corrupt or truncated file.
+ * kj_last_kernel_ms() then gives the device time of the inflate kernel. */
+int kj_debug_inflate_bgzf(kj_ctx *ctx, const uint8_t *file_bytes, uint64_t n, uint8_t *out, uint64_t out_cap, uint64_t *out_n,
+                          uint64_t *first_bad_offset);
 
 #ifdef __cplusplus
 }

@@ -102,6 +102,9 @@ def lib():
         L.kj_check_errors.argtypes = [C.c_void_p]
         L.kj_launch_geometry.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.kj_version.restype = C.c_int
+        if hasattr(L, "kj_debug_inflate_bgzf"):
+            L.kj_files_device_inflated_bytes.restype = C.c_uint64; L.kj_files_device_inflated_bytes.argtypes = [C.c_void_p]
+            L.kj_debug_inflate_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         _lib = L
     return _lib
 
@@ -295,11 +298,28 @@ class Classifier:
         return self.counts(nonzero=False)[0]
 
     def classify_files(self, in1, in2=None, out_path=None, verbose=False):
-        """FASTA/FASTQ(.gz) files -> kaiju output file, parsed / classified / formatted on the device.  Returns (reads, classified)."""
+        """FASTA/FASTQ(.gz) files -> kaiju output file, parsed / classified / formatted on the device (blocked gzip, BGZF, is inflated
+        there too; other gzip by zlib on the host).  Returns (reads, classified)."""
         n = C.c_uint64(); k = C.c_uint64()
         _check(lib().kj_classify_files(self._ctx, in1.encode(), in2.encode() if in2 else None, out_path.encode() if out_path else None,
                                        1 if verbose else 0, C.byref(n), C.byref(k)))
         return int(n.value), int(k.value)
+
+    @property
+    def files_device_inflated_bytes(self):
+        """Bytes of text the device inflated in the last classify_files call (0 for plain text and for gzip that zlib inflated)."""
+        return int(lib().kj_files_device_inflated_bytes(self._ctx))
+
+    def debug_inflate_bgzf(self, data, out_cap=None):
+        """Test hook: the text of a whole BGZF file (bytes) from the inflate kernel.  A bad block raises KaijuError; its compressed offset is
+        in the exception's bad_offset."""
+        buf = np.frombuffer(bytes(data), dtype=np.uint8) if len(data) else np.zeros(1, np.uint8)
+        cap = int(out_cap) if out_cap is not None else 64 * len(data) + 65536
+        out = np.empty(max(cap, 1), dtype=np.uint8); n = C.c_uint64(); bad = C.c_uint64()
+        rc = lib().kj_debug_inflate_bgzf(self._ctx, buf.ctypes.data, len(data), out.ctypes.data, cap, C.byref(n), C.byref(bad))
+        if rc != 0:
+            e = KaijuError("kaiju_b200 error %d: %s" % (rc, lib().kj_last_error().decode())); e.bad_offset = int(bad.value); raise e
+        return out[:n.value].tobytes()
 
     # ---- per-taxon read counts accumulated in HBM by the successful classify calls (input of kaiju2table)
     def counts_reset(self):

@@ -267,7 +267,7 @@ int main(int argc, char** argv) {
 
     // parsing, classification and output formatting all run on the device; the host moves bytes (kj_ingest.h).
     // Comma-separated lists for -i / -j / -o process several data sets against the index loaded once per device (kaiju-multi.cpp:220-330).
-    struct Done { uint64_t n_reads = 0, n_classified = 0; double secs = 0; std::vector<uint64_t> ids, counts; };
+    struct Done { uint64_t n_reads = 0, n_classified = 0, inflated = 0; double secs = 0; std::vector<uint64_t> ids, counts; };
     std::vector<Done> done(l1.size()); std::atomic<size_t> next(0); std::mutex mu; std::string err;
     std::vector<std::thread> workers;
     for (size_t d = 0; d < ctxs.size(); d++) workers.emplace_back([&, d] {
@@ -280,6 +280,7 @@ int main(int argc, char** argv) {
             if (rc == KJ_OK && verbose && fmi) run_verbose(ctx, fmi, P, l1[k], paired ? l2[k] : std::string(), lo.empty() ? std::string() : lo[k], r.n_reads, r.n_classified);
             else if (rc == KJ_OK) rc = kj_classify_files(ctx, l1[k].c_str(), paired ? l2[k].c_str() : nullptr, lo.empty() ? nullptr : lo[k].c_str(), verbose ? 1 : 0, &r.n_reads, &r.n_classified);
             r.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+            r.inflated = kj_files_device_inflated_bytes(ctx);
             if (rc == KJ_OK && !table_fn.empty()) { r.ids.resize(kj_counts_size(ctx)); r.counts.resize(r.ids.size()); rc = kj_counts_get(ctx, r.ids.data(), r.counts.data()); }
             if (rc != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); return; }
         }
@@ -293,6 +294,7 @@ int main(int argc, char** argv) {
             if (kj_table_write(done[k].ids.data(), done[k].counts.data(), done[k].ids.size(), nodes_fn.c_str(), names_fn.c_str(), label.c_str(), &to, table_fn.c_str(), k > 0) != KJ_OK) die(kj_last_error());
         }
         if (verbose || getenv("KJ_CLI_TIMING")) fprintf(stderr, "%s: %llu reads, %llu classified, %.4f s from the first byte read to the last byte written\n", l1[k].c_str(), (unsigned long long)done[k].n_reads, (unsigned long long)done[k].n_classified, done[k].secs);
+        if (getenv("KJ_CLI_TIMING")) fprintf(stderr, "%s: %llu bytes of text inflated on the device (BGZF input; 0: plain text, or gzip inflated by zlib on the host)\n", l1[k].c_str(), (unsigned long long)done[k].inflated);
     }
     for (kj_ctx* ctx : ctxs) kj_destroy(ctx);
     if (fmi) kj_fmi_free(fmi);

@@ -12,7 +12,7 @@
 
 std::string& kj_err() { static thread_local std::string e; return e; }
 extern "C" const char* kj_last_error(void) { return kj_err().c_str(); }
-extern "C" int kj_version(void) { return 100; }
+extern "C" int kj_version(void) { return 101; }
 
 // ------------------------------------------------------------------------------------------------
 // .fmi  (written by kaiju-mkfmi, mkfmi.c:68-77): BWT header (bwt.c:40-45), suffix-array header + body

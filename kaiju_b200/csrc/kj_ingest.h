@@ -7,7 +7,8 @@
 //   newline positions (count + scan + scatter) -> per-line classification (header / sequence / ignored), letters and
 //   trimmed-name lengths (one warp per line) -> scans over lines -> packed sequences + offsets + names blob ->
 //   kj_classify_kernel -> per-record output line lengths -> scan -> formatted "C\tname\ttaxid..." text.
-// The host only moves bytes (kj_classify_files): reader threads (one per file: page cache -> two pinned buffers -> ring of device staging buffers),
+// The host only moves bytes (kj_classify_files): reader threads (one per file: page cache -> two pinned buffers -> ring of device staging buffers;
+// blocked gzip (BGZF) is inflated on the way by kj_inflate_kernel, other gzip by zlib on the reader thread),
 // a parser thread (staged chunks -> batches of device text -> the kernels above on a high-priority stream; the incomplete record at the end of a batch is
 // carried over on the device), the calling thread (two classification lanes: launch batch k+1 while batch k runs, count / format / copy out batch k-1) and
 // a writer thread.  Record rules beyond the happy path (kaiju.cpp:288-404): file type = first character of the first non-empty line, empty lines between
@@ -20,6 +21,7 @@
 #include <condition_variable>
 #include <deque>
 #include <mutex>
+#include "kj_inflate.h"
 
 // ------------------------------------------------------------------------------------------------
 // device-wide exclusive scan of uint32 (in place); total -> *total.  Tile = 256 threads x 8 elements.
@@ -376,10 +378,14 @@ static int kj_parse_sides(int sm_count, KjParsed* Ps, KjBatchSide* Os, int nfile
     return KJ_OK;
 }
 
+static inline double kj_ms_since(std::chrono::steady_clock::time_point& t) { const auto n = std::chrono::steady_clock::now(); const double d = std::chrono::duration<double, std::milli>(n - t).count(); t = n; return d; }
 // One I/O chunk of an input file, already on its way to the device: slot of the reader's staging ring + the event of its copy
 struct KjStaged { int slot = -1; size_t n = 0; bool eof = false; char last = 0; cudaEvent_t ev = nullptr; std::string error; };
 // Per input file: gz (zlib, one thread) or plain (a pool of pread() threads) -> two alternating pinned buffers -> host-to-device copies on the
 // reader's own stream into a ring of device staging buffers.  The parser only ever sees device memory; the pinned footprint is two chunks.
+// BGZF (a gzip file whose first member carries the "BC" extra subfield): the compressed bytes are read like a plain file's, the block chain is
+// walked on the host and the blocks are inflated on the device straight into the ring slot a plain chunk would have been copied to; a later
+// member that is no BGZF block sends the rest of the file to zlib.
 struct KjFileReader {
     gzFile fp = nullptr; int fd = -1; uint64_t file_off = 0; std::string path; size_t chunk = 0; int device = 0; KjPinnedPool* pinned = nullptr;
     char* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; bool pin_busy[2] = {false, false}; cudaStream_t stream = nullptr;
@@ -389,6 +395,11 @@ struct KjFileReader {
     static constexpr size_t SLICE = 1u << 20;
     std::vector<std::thread> workers; std::mutex wmu; std::condition_variable wcv, wdone; char* wbuf = nullptr; size_t wnext = 0, wslices = 0, wleft = 0; uint64_t wgen = 0; bool wstop = false, werr = false;
     std::vector<size_t> wgot;
+    // BGZF: bytes read per round (a whole block always fits), size of a ring slot, most blocks per round; the compressed bytes, the block table
+    // and the blocks' status words of a round share one pinned buffer and one device buffer (two of each: one round is in flight while the next is read)
+    bool bgzf = false; size_t rchunk = 0, slot_bytes = 0, max_blocks = 0, tab_off = 0, st_off = 0, last_off = 0, zbytes = 0;
+    char* zpin[2] = {nullptr, nullptr}; KjDevBuf zdev[2]; cudaStream_t zstream = nullptr; std::vector<KjBgzfBlock> table;
+    uint64_t inflated = 0; char last_byte = 0; double tm_read = 0, tm_inflate = 0;
     void worker() {
         uint64_t seen = 0;
         for (;;) {
@@ -399,7 +410,7 @@ struct KjFileReader {
             while (wgen == gen && wnext < wslices) {
                 const size_t sl = wnext++; char* b = wbuf; const uint64_t base = file_off;
                 lk.unlock();
-                const size_t o = sl * SLICE, want = std::min(SLICE, chunk - o); size_t g = 0; bool bad = false;
+                const size_t o = sl * SLICE, want = std::min(SLICE, rchunk - o); size_t g = 0; bool bad = false;
                 while (g < want) { const ssize_t r = ::pread(fd, b + o + g, want - g, (off_t)(base + o + g)); if (r < 0) { bad = true; break; } if (r == 0) break; g += (size_t)r; }
                 lk.lock();
                 wgot[sl] = g; if (bad) werr = true;
@@ -409,11 +420,17 @@ struct KjFileReader {
         }
     }
     int open(const std::string& p, size_t chunk_bytes, int depth, int device_, KjPinnedPool* pp) {
-        path = p; chunk = chunk_bytes; device = device_; pinned = pp; stop = false; wstop = false; file_off = 0;
+        path = p; chunk = chunk_bytes; device = device_; pinned = pp; stop = false; wstop = false; file_off = 0; inflated = 0; last_byte = 0; tm_read = tm_inflate = 0;
         fd = ::open(p.c_str(), O_RDONLY);
         if (fd < 0) { kj_err() = "Could not open file " + p; return KJ_ERR_IO; }
-        unsigned char magic[2] = {0, 0}; const ssize_t got = ::pread(fd, magic, 2, 0);
-        if (got == 2 && magic[0] == 0x1f && magic[1] == 0x8b) {             // gzip: inflate through zlib; everything else is read as it is
+        std::vector<uint8_t> head(65536); const ssize_t got = ::pread(fd, head.data(), head.size(), 0); const unsigned char* magic = head.data();
+        {   // BGZF is what the first member says it is: a gzip header with the "BC" subfield (its whole block lies within the first 64 KiB)
+            table.clear(); const int st = got > 0 ? kj_bgzf_walk(head.data(), (size_t)got, 0, 1, 0, 0, table).stop : KJ_BGZF_GARBAGE;
+            bgzf = !table.empty() || st == KJ_BGZF_PARTIAL;
+        }
+        rchunk = bgzf ? std::max<size_t>(chunk, 65536) : chunk; slot_bytes = rchunk + 16;
+        max_blocks = rchunk / 1024 + 64; tab_off = (rchunk + 63) & ~(size_t)63; st_off = tab_off + max_blocks * sizeof(KjBgzfBlock); last_off = st_off + max_blocks * 4; zbytes = last_off + 16;
+        if (!bgzf && got >= 2 && magic[0] == 0x1f && magic[1] == 0x8b) {             // other gzip: inflate through zlib; everything else is read as it is
             ::close(fd); fd = -1; fp = gzopen(p.c_str(), "rb");
             if (!fp) { kj_err() = "Could not open file " + p; return KJ_ERR_IO; }
             gzbuffer(fp, 1 << 20);
@@ -421,7 +438,7 @@ struct KjFileReader {
             posix_fadvise(fd, 0, 0, POSIX_FADV_SEQUENTIAL);
             unsigned nt = std::max(2u, std::min(8u, std::thread::hardware_concurrency() / 4u));
             if (const char* v = getenv("KJ_IO_THREADS")) { const long x = atol(v); if (x >= 1 && x <= 64) nt = (unsigned)x; }      // tuning hook
-            wgot.assign((chunk + SLICE - 1) / SLICE, 0);
+            wgot.assign((rchunk + SLICE - 1) / SLICE, 0);
             for (unsigned t = 0; t < nt; t++) workers.emplace_back([this] { worker(); });
         }
         if ((int)ring.size() != depth) { ring.clear(); ring.resize((size_t)depth); }
@@ -429,12 +446,95 @@ struct KjFileReader {
         th = std::thread([this] { run(); });
         return KJ_OK;
     }
+    // one round of the worker pool: the rchunk bytes at file_off (fewer at the end of the file) into b.  false: read error
+    bool read_round(char* b, size_t& got, bool& eof) {
+        const size_t ns = (rchunk + SLICE - 1) / SLICE; got = 0; eof = false;
+        {
+            std::unique_lock<std::mutex> lk(wmu);
+            wbuf = b; wnext = 0; wslices = ns; wleft = ns; werr = false; wgen++;
+            wcv.notify_all();
+            wdone.wait(lk, [&] { return wleft == 0; });
+            wslices = 0;
+        }
+        if (werr) return false;
+        for (size_t sl = 0; sl < ns; sl++) {
+            got += wgot[sl];
+            if (wgot[sl] < std::min(SLICE, rchunk - sl * SLICE)) { eof = true; break; }          // short slice = end of file (later slices read nothing)
+        }
+        if (got == rchunk && !eof) { char probe; if (::pread(fd, &probe, 1, (off_t)(file_off + rchunk)) == 0) eof = true; }
+        return true;
+    }
+    // The BGZF blocks of the file, round by round.  false: the file is done (its last chunk or an error is queued); true: a gzip member that is no
+    // BGZF block starts at file_off, and zlib (fp) reads the rest.
+    bool run_bgzf() {
+        struct Flight { KjStaged ck; int pb = 0; size_t nblk = 0; uint64_t off = 0; bool on = false; } prev, cur;
+        auto finish = [&](Flight& f) -> bool {      // the round's blocks are inflated and good: its chunk goes to the parser
+            if (!f.on) return true;
+            auto t0 = std::chrono::steady_clock::now();
+            if (cudaEventSynchronize(f.ck.ev) != cudaSuccess) { fail("inflating " + path + " failed on the device"); return false; }
+            tm_inflate += kj_ms_since(t0);
+            const uint32_t* st = (const uint32_t*)(zpin[f.pb] + st_off); const KjBgzfBlock* tb = (const KjBgzfBlock*)(zpin[f.pb] + tab_off);
+            for (size_t i = 0; i < f.nblk; i++) if (st[i]) {
+                fail("corrupt BGZF block in file " + path + " at compressed offset " + std::to_string(f.off + tb[i].in_off - tb[i].hdr) + ": " + kj_inflate_strerror(st[i])); return false; }
+            if (f.ck.n) last_byte = zpin[f.pb][last_off];
+            f.ck.last = last_byte; f.on = false;
+            { std::lock_guard<std::mutex> lk(mu); ready.push_back(f.ck); }
+            cv.notify_all(); return true;
+        };
+        if (!zstream) { int lo = 0, hi = 0;      // beside the parse stream: the inflate kernel, too, has to find room next to the persistent classify grid
+            if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess || cudaStreamCreateWithPriority(&zstream, cudaStreamNonBlocking, hi) != cudaSuccess) { fail("cudaStreamCreate failed"); return false; } }
+        for (uint64_t it = 0;; it++) {
+            const int pb = (int)(it & 1);          // the round that used this pair of buffers has been finished one round ago
+            if (!zpin[pb]) { zpin[pb] = pinned->get(zbytes); if (!zpin[pb]) { fail("cudaMallocHost failed"); return false; } }
+            if (zdev[pb].grow(zbytes) != KJ_OK) { fail("cudaMalloc failed (compressed staging)"); return false; }
+            char* b = zpin[pb]; size_t got = 0; bool ceof = false;
+            auto t0 = std::chrono::steady_clock::now();
+            if (!read_round(b, got, ceof)) { fail("read error in file " + path); return false; }
+            tm_read += kj_ms_since(t0);
+            table.clear();
+            const KjBgzfWalk w = kj_bgzf_walk((const uint8_t*)b, got, slot_bytes - 16, max_blocks, 0, 0, table);
+            bool eof = false, to_zlib = false;
+            if (w.stop == KJ_BGZF_END) eof = ceof;
+            else if (w.stop == KJ_BGZF_GARBAGE) eof = true;                  // zlib, too, ignores what follows the last member
+            else if (w.stop == KJ_BGZF_FOREIGN) to_zlib = true;
+            else if (w.stop == KJ_BGZF_BAD) { fail("corrupt BGZF header in file " + path + " at compressed offset " + std::to_string(file_off + w.consumed)); return false; }
+            else if (w.stop == KJ_BGZF_PARTIAL && (ceof || w.consumed == 0)) { fail("truncated BGZF block in file " + path + " at compressed offset " + std::to_string(file_off + w.consumed)); return false; }
+            cur = Flight(); cur.pb = pb; cur.nblk = table.size(); cur.off = file_off; cur.on = true; cur.ck.n = (size_t)w.out_bytes; cur.ck.eof = eof;
+            {   // a free staging buffer on the device
+                std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || !free_slots.empty(); }); if (stop) return false;
+                cur.ck.slot = free_slots.front(); free_slots.pop_front();
+            }
+            if (kj_need(ring[cur.ck.slot], slot_bytes) != KJ_OK) { fail("cudaMalloc failed (staging ring)"); return false; }
+            if (cur.nblk) {
+                memcpy(b + tab_off, table.data(), cur.nblk * sizeof(KjBgzfBlock));
+                char* d = zdev[pb].as<char>(); bool ok = true;
+                ok = ok && cudaMemcpyAsync(d, b, w.consumed, cudaMemcpyHostToDevice, zstream) == cudaSuccess;
+                ok = ok && cudaMemcpyAsync(d + tab_off, b + tab_off, cur.nblk * sizeof(KjBgzfBlock), cudaMemcpyHostToDevice, zstream) == cudaSuccess;
+                if (ok) kj_inflate_kernel<<<(unsigned)((cur.nblk + KJ_INF_WARPS - 1) / KJ_INF_WARPS), KJ_INF_WARPS * 32, 0, zstream>>>((const uint8_t*)d, (const KjBgzfBlock*)(d + tab_off), (uint32_t)cur.nblk,
+                                                                                                                                      ring[cur.ck.slot].as<uint8_t>(), (uint32_t*)(d + st_off));
+                ok = ok && cudaGetLastError() == cudaSuccess;
+                ok = ok && cudaMemcpyAsync(b + st_off, d + st_off, cur.nblk * 4, cudaMemcpyDeviceToHost, zstream) == cudaSuccess;
+                if (cur.ck.n) ok = ok && cudaMemcpyAsync(b + last_off, ring[cur.ck.slot].as<char>() + cur.ck.n - 1, 1, cudaMemcpyDeviceToHost, zstream) == cudaSuccess;
+                if (!ok) { fail("launching the inflate kernel failed"); return false; }
+            }
+            cudaEventRecord(ring_ev[cur.ck.slot], zstream); cur.ck.ev = ring_ev[cur.ck.slot];
+            file_off += w.consumed; inflated += w.out_bytes;
+            if (!finish(prev)) return false;
+            prev = cur;
+            if (!eof && !to_zlib) continue;
+            if (!finish(prev) || eof) return false;
+            if (::lseek(fd, (off_t)file_off, SEEK_SET) < 0 || !(fp = gzdopen(fd, "rb"))) { fail("Could not open file " + path); return false; }
+            fd = -1; gzbuffer(fp, 1 << 20);
+            return true;
+        }
+    }
     void fail(const std::string& what) { KjStaged e; e.error = what; { std::lock_guard<std::mutex> lk(mu); ready.push_back(e); } cv.notify_all(); }
     void run() {
         if (cudaSetDevice(device) != cudaSuccess) { fail("cudaSetDevice failed"); return; }
         if (!stream && cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) { fail("cudaStreamCreate failed"); return; }
         while (ring_ev.size() < ring.size()) { cudaEvent_t e; if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) { fail("cudaEventCreate failed"); return; } ring_ev.push_back(e); }
-        char prev_last = 0;
+        if (bgzf && !run_bgzf()) return;
+        char prev_last = last_byte;
         for (uint64_t it = 0;; it++) {
             const int pb = (int)(it & 1);
             if (!pin[pb]) {       // allocated here, next to the running pipeline, not before it starts
@@ -444,20 +544,7 @@ struct KjFileReader {
             if (pin_busy[pb]) { cudaEventSynchronize(pin_ev[pb]); pin_busy[pb] = false; }     // the copy that read this buffer two chunks ago
             char* b = pin[pb]; KjStaged ck; size_t got = 0;
             if (fd >= 0) {
-                const size_t ns = (chunk + SLICE - 1) / SLICE;
-                {
-                    std::unique_lock<std::mutex> lk(wmu);
-                    wbuf = b; wnext = 0; wslices = ns; wleft = ns; werr = false; wgen++;
-                    wcv.notify_all();
-                    wdone.wait(lk, [&] { return wleft == 0; });
-                    wslices = 0;
-                }
-                if (werr) ck.error = "read error in file " + path;
-                else for (size_t sl = 0; sl < ns; sl++) {
-                    got += wgot[sl];
-                    if (wgot[sl] < std::min(SLICE, chunk - sl * SLICE)) { ck.eof = true; break; }          // short slice = end of file (later slices read nothing)
-                }
-                if (got == chunk && !ck.eof && ck.error.empty()) { char probe; if (::pread(fd, &probe, 1, (off_t)(file_off + chunk)) == 0) ck.eof = true; }
+                if (!read_round(b, got, ck.eof)) ck.error = "read error in file " + path;
                 file_off += got;
             } else while (got < chunk) {
                 const ssize_t r = (ssize_t)gzread(fp, b + got, (unsigned)std::min<size_t>(chunk - got, 1u << 30));
@@ -471,7 +558,7 @@ struct KjFileReader {
                 std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || !free_slots.empty(); }); if (stop) return;
                 ck.slot = free_slots.front(); free_slots.pop_front();
             }
-            if (kj_need(ring[ck.slot], chunk + 16) != KJ_OK) { fail("cudaMalloc failed (staging ring)"); return; }
+            if (kj_need(ring[ck.slot], slot_bytes) != KJ_OK) { fail("cudaMalloc failed (staging ring)"); return; }
             if (got && cudaMemcpyAsync(ring[ck.slot].p, b, got, cudaMemcpyHostToDevice, stream) != cudaSuccess) { fail("cudaMemcpyAsync failed"); return; }
             cudaEventRecord(ring_ev[ck.slot], stream); cudaEventRecord(pin_ev[pb], stream); pin_busy[pb] = true; ck.ev = ring_ev[ck.slot];
             const bool last = ck.eof;
@@ -489,12 +576,14 @@ struct KjFileReader {
         for (auto& w : workers) if (w.joinable()) w.join();
         workers.clear();
         if (stream) cudaStreamSynchronize(stream);
+        if (zstream) cudaStreamSynchronize(zstream);
+        for (int k = 0; k < 2; k++) { if (zpin[k]) pinned->put(zpin[k], zbytes); zpin[k] = nullptr; }
         if (fp) gzclose(fp); fp = nullptr;
         if (fd >= 0) ::close(fd); fd = -1;
         for (int k = 0; k < 2; k++) { if (pin[k]) pinned->put(pin[k], chunk); pin[k] = nullptr; pin_busy[k] = false; if (pin_ev[k]) cudaEventDestroy(pin_ev[k]); pin_ev[k] = nullptr; }
         ready.clear(); free_slots.clear(); wgen = 0; wslices = 0; wnext = 0; wleft = 0;
     }
-    void release() { for (auto e : ring_ev) cudaEventDestroy(e); ring_ev.clear(); if (stream) cudaStreamDestroy(stream); stream = nullptr; }
+    void release() { for (auto e : ring_ev) cudaEventDestroy(e); ring_ev.clear(); if (stream) cudaStreamDestroy(stream); stream = nullptr; if (zstream) cudaStreamDestroy(zstream); zstream = nullptr; }
 };
 struct KjWriter {   // ordered output: pinned buffers filled by D2H copies, written by one thread
     FILE* out = nullptr; bool own = false; std::vector<char*> pool; size_t cap = 0; int nbuf = 3; std::deque<std::pair<char*, size_t>> ready; std::deque<char*> free_;
@@ -541,6 +630,7 @@ struct KjFilesState {
     // parser thread -> classifying thread: filled slots in order; slots come back when their batch has been written
     std::mutex mu; std::condition_variable cv; std::deque<int> filled; int n_free = KJ_FILE_SLOTS; bool abort = false; std::thread parser;
     std::string fn[2], perr; int prc = KJ_OK;                 // input names; the parser thread's error
+    uint64_t dev_inflated = 0;                                // bytes of text the inflate kernel produced in the last call
     uint64_t parse_launches = 0; double tm[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; uint64_t nbatches = 0;
     void end_call() {      // threads, files and in-flight copies of one call
         { std::lock_guard<std::mutex> lk(mu); abort = true; } cv.notify_all();
@@ -559,8 +649,6 @@ struct KjFilesState {
     }
 };
 static void kj_files_state_free(KjFilesState* S) { if (!S) return; S->end_call(); S->release(); delete S; }
-
-static inline double kj_ms_since(std::chrono::steady_clock::time_point& t) { const auto n = std::chrono::steady_clock::now(); const double d = std::chrono::duration<double, std::milli>(n - t).count(); t = n; return d; }
 
 // Parser thread: staged file chunks -> device text -> packed reads, names and offsets of the complete records, one KjBatch per round.
 // Stage 1 of the pipeline: while the caller's thread classifies and formats earlier batches on its streams, this thread assembles and parses the
@@ -775,6 +863,8 @@ static int kj_classify_files_impl(kj_ctx* c, KjFilesState& S, const char* in1, c
     for (int l = 0; l < 2; l++) { unsigned long long v = 0; CK(cudaMemcpy(&v, (char*)S.lane[l].totals.p + 16, 8, cudaMemcpyDeviceToHost)); n_class += v; }
     if (ftrace) fprintf(stderr, "KJ_FILES_TRACE batches %llu  parser: slot-wait %.1f  chunk-wait+append %.1f  parse+carry %.1f | classifier: batch-wait %.1f  classify-wait %.1f  format+d2h %.1f ms\n",
                         (unsigned long long)S.nbatches, S.tm[0], S.tm[1], S.tm[3], S.tm[5], S.tm[6], S.tm[7]);
+    if (ftrace) for (int f = 0; f < S.nfiles; f++) if (S.rd[f].bgzf)
+        fprintf(stderr, "KJ_FILES_TRACE reader %d (BGZF): read %.1f  inflate-wait %.1f ms  inflated %llu bytes on the device\n", f, S.rd[f].tm_read, S.rd[f].tm_inflate, (unsigned long long)S.rd[f].inflated);
     if (n_reads_out) *n_reads_out = n_reads; if (n_class_out) *n_class_out = n_class;
     return KJ_OK;
 }
@@ -785,10 +875,45 @@ extern "C" int kj_classify_files(kj_ctx* c, const char* in1, const char* in2, co
     CK(cudaSetDevice(c->device));
     if (!c->files) c->files.reset(new KjFilesState());
     KjFilesState* S = c->files.get();
+    S->dev_inflated = 0;
     int rc = kj_classify_files_impl(c, *S, in1, in2, out_path, verbose, n_reads, n_classified);
     const std::string keep = kj_err();
+    for (int f = 0; f < 2; f++) if (S->rd_open[f]) S->dev_inflated += S->rd[f].inflated;
     cudaStreamSynchronize(c->slot[0].stream); cudaStreamSynchronize(c->slot[1].stream);
     S->end_call();
     if (rc) { cudaMemset(c->err.p, 0, 4); kj_err() = keep; } else if (S->wr.failed) { kj_err() = "write error on the output file"; rc = KJ_ERR_IO; }
     return rc;
+}
+
+extern "C" uint64_t kj_files_device_inflated_bytes(const kj_ctx* c) { return c && c->files ? c->files->dev_inflated : 0; }
+
+// test hook: a whole BGZF file in host memory through the header walk and the inflate kernel of the file pipeline
+extern "C" int kj_debug_inflate_bgzf(kj_ctx* c, const uint8_t* file_bytes, uint64_t n, uint8_t* out, uint64_t out_cap, uint64_t* out_n, uint64_t* first_bad_offset) {
+    if (!c || (!file_bytes && n) || !out_n || !first_bad_offset) { kj_err() = "kj_debug_inflate_bgzf: null argument"; return KJ_ERR_ARG; }
+    CK(cudaSetDevice(c->device));
+    *out_n = 0; *first_bad_offset = 0;
+    std::vector<KjBgzfBlock> table; const KjBgzfWalk w = kj_bgzf_walk(file_bytes, (size_t)n, ~0ull, ~(size_t)0, 0, 0, table);
+    if (w.stop != KJ_BGZF_END && w.stop != KJ_BGZF_GARBAGE) {
+        *first_bad_offset = w.consumed; kj_err() = std::string(w.stop == KJ_BGZF_PARTIAL ? "truncated BGZF block" : w.stop == KJ_BGZF_FOREIGN ? "not a BGZF block" : "corrupt BGZF header") + " at compressed offset " + std::to_string(w.consumed);
+        return KJ_ERR_IO;
+    }
+    if (w.out_bytes > out_cap || (w.out_bytes && !out)) { kj_err() = "kj_debug_inflate_bgzf: the output buffer is too small"; return KJ_ERR_ARG; }
+    if (table.empty()) return KJ_OK;
+    if (table.size() >= (1ull << 32)) { kj_err() = "kj_debug_inflate_bgzf: too many blocks"; return KJ_ERR_UNSUPPORTED; }
+    KjDevBuf comp, tab, text, status; int rc; const uint32_t nblk = (uint32_t)table.size(); std::vector<uint32_t> st(nblk);
+    if ((rc = comp.grow(w.consumed)) || (rc = tab.grow(nblk * sizeof(KjBgzfBlock))) || (rc = text.grow(w.out_bytes + 16)) || (rc = status.grow((size_t)nblk * 4))) return rc;
+    cudaStream_t s = c->slot[0].stream;
+    CK(cudaMemcpyAsync(comp.p, file_bytes, w.consumed, cudaMemcpyHostToDevice, s)); CK(cudaMemcpyAsync(tab.p, table.data(), nblk * sizeof(KjBgzfBlock), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(c->ev_a, s));
+    kj_inflate_kernel<<<(nblk + KJ_INF_WARPS - 1) / KJ_INF_WARPS, KJ_INF_WARPS * 32, 0, s>>>(comp.as<uint8_t>(), tab.as<KjBgzfBlock>(), nblk, text.as<uint8_t>(), status.as<uint32_t>());
+    CK(cudaGetLastError()); c->launches++;
+    CK(cudaEventRecord(c->ev_b, s));
+    CK(cudaMemcpyAsync(st.data(), status.p, (size_t)nblk * 4, cudaMemcpyDeviceToHost, s));
+    if (w.out_bytes) CK(cudaMemcpyAsync(out, text.p, w.out_bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (uint32_t i = 0; i < nblk; i++) if (st[i]) {
+        *first_bad_offset = table[i].in_off - table[i].hdr;
+        kj_err() = "corrupt BGZF block at compressed offset " + std::to_string(*first_bad_offset) + ": " + kj_inflate_strerror(st[i]); return KJ_ERR_IO;
+    }
+    *out_n = w.out_bytes; return KJ_OK;
 }
