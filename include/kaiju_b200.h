@@ -196,9 +196,29 @@ int kj_device_count(void);                        /* number of usable CUDA devic
  * gzip input: a blocked gzip file (BGZF, what `bgzip` writes: the first member carries the "BC" extra subfield) is inflated on the device, one
  * block per warp, CRC-32 and length of every block checked there; only the compressed bytes cross to the device.  Should a later member of
  * such a file not be a BGZF block, zlib reads the rest from there.  Every other gzip file is inflated by zlib on one host thread per file.
- * A corrupt or truncated BGZF block is KJ_ERR_IO, and kj_last_error() names the file and the block's offset in it. */
-int kj_classify_files(kj_ctx *ctx, const char *in1, const char *in2, const char *out_path, int verbose,
+ * A corrupt or truncated BGZF block is KJ_ERR_IO, and kj_last_error() names the file and the block's offset in it.
+ * `format` is one of the KJ_OUT_* line formats below (0 and 1 are the former `verbose` = 0 / 1).  Format 2 needs the KJ_STR_ACCESSION table,
+ * formats 3 and 4 the KJ_STR_TAXON table and a context in params.name_mode (kj_set_output_strings); otherwise KJ_ERR_ARG before anything is
+ * read.  With name_mode and input_is_protein the reader follows kaijup (kaijup.cpp:227-262): names are kept whole and the file type is the
+ * first character of the first line.  The fragment strings of formats 2 and 4 are written to a buffer of at most 512 MB per pipeline lane;
+ * a batch that needs more is classified in consecutive launches.  A read whose strings exceed 32 x (residues + 2) + 64 bytes (residues: of
+ * its batch's longest mate) fails the call with KJ_ERR_OVERFLOW; n_classified_out counts the "C" lines. */
+#define KJ_OUT_KAIJU 0        /* "C\t<name>\t<taxid>" / "U\t<name>\t0"                                                   */
+#define KJ_OUT_KAIJU_IDS 1    /* + "\t<best>\t<id>,...," on C lines                                                        */
+#define KJ_OUT_KAIJU_V 2      /* the seven columns of `kaiju -v`: + best, taxon-id set, accession set, fragment strings     */
+#define KJ_OUT_NAMES 3        /* kaijux / kaijup: "C\t<name>\t<best>\t<label>,...,\t"; "U\t<name>\t0" (stopped by the front-end
+                                 gate) / "U\t<name>" (no match)                                                              */
+#define KJ_OUT_NAMES_V 4      /* kaijux -v / kaijup -v: as 3 with the fragment strings after the last tab                   */
+int kj_classify_files(kj_ctx *ctx, const char *in1, const char *in2, const char *out_path, int format,
                       uint64_t *n_reads_out, uint64_t *n_classified_out);
+/* The strings kj_classify_files prints in place of numbers: string k = blob[off[k], off[k + 1]), off has n + 1 entries.
+ *   KJ_STR_ACCESSION: n = number of distinct accessions, string r = accession of rank r (kj_index_view.seq_accession, column 6 of -v)
+ *   KJ_STR_TAXON:     n = kj_counts_size(ctx) - 1, string k = label printed for the taxon of dense index k (kj_counts_get order)
+ * The table is copied to where the index keeps its suffix-array taxa (HBM, or the host tier of kj_create_tiered) and counts in
+ * kj_index_bytes / kj_index_host_bytes; setting a kind again replaces it; kj_destroy frees it.  KJ_ERR_NOMEM names the bytes. */
+#define KJ_STR_ACCESSION 0
+#define KJ_STR_TAXON 1
+int kj_set_output_strings(kj_ctx *ctx, int kind, const char *blob, const uint64_t *off, uint64_t n);
 /* Bytes of text the device inflated in the last kj_classify_files call of the context (both input files; 0 for plain and zlib input). */
 uint64_t kj_files_device_inflated_bytes(const kj_ctx *ctx);
 

@@ -17,6 +17,9 @@ MAX_READ_LEN = 16383           # default read-length limit, bases per mate (incl
 MAX_LONG_READ_LEN = 1048575     # the highest limit Classifier.set_max_read_len accepts (KJ_MAX_LONG_READ_LEN)
 
 MEM, GREEDY = 0, 1
+# output formats of Classifier.classify_files (KJ_OUT_*) and the string tables of set_output_strings (KJ_STR_*)
+OUT_KAIJU, OUT_KAIJU_IDS, OUT_KAIJU_V, OUT_NAMES, OUT_NAMES_V = 0, 1, 2, 3, 4
+STR_ACCESSION, STR_TAXON = 0, 1
 
 
 class KjParams(C.Structure):
@@ -105,6 +108,9 @@ def lib():
         if hasattr(L, "kj_debug_inflate_bgzf"):
             L.kj_files_device_inflated_bytes.restype = C.c_uint64; L.kj_files_device_inflated_bytes.argtypes = [C.c_void_p]
             L.kj_debug_inflate_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        if hasattr(L, "kj_set_output_strings"):
+            L.kj_set_output_strings.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64]
+        L.kj_fmi_accession.restype = C.c_char_p; L.kj_fmi_accession.argtypes = [C.c_void_p, C.c_uint32]
         _lib = L
     return _lib
 
@@ -163,6 +169,21 @@ def write_native_index(fmi_path, nodes_path, out_path):
             _check(L.kj_native_index_write(C.byref(iv), C.byref(tv), out_path.encode()))
         finally:
             L.kj_nodes_free(nodes)
+    finally:
+        L.kj_fmi_free(fmi)
+
+
+def fmi_accessions(fmi_path):
+    """The distinct accessions of a .fmi index by rank (what classify_files prints in column 6 of OUT_KAIJU_V; set_output_strings)."""
+    L = lib(); fmi = C.c_void_p(); iv = KjIndexView()
+    _check(L.kj_fmi_load(fmi_path.encode(), C.byref(fmi)))
+    try:
+        L.kj_fmi_view(fmi, C.byref(iv))
+        if not iv.seq_accession:
+            return []
+        ranks = np.ctypeslib.as_array(C.cast(iv.seq_accession, C.POINTER(C.c_uint32)), shape=(int(iv.nseq),))
+        n = int(ranks[ranks != 0xffffffff].max()) + 1 if (ranks != 0xffffffff).any() else 0
+        return [L.kj_fmi_accession(fmi, r) or b"" for r in range(n)]
     finally:
         L.kj_fmi_free(fmi)
 
@@ -297,13 +318,25 @@ class Classifier:
         """NCBI taxon id of every dense taxon index (the id list of counts(); the last entry, 0, stands for unclassified)."""
         return self.counts(nonzero=False)[0]
 
-    def classify_files(self, in1, in2=None, out_path=None, verbose=False):
+    def classify_files(self, in1, in2=None, out_path=None, verbose=False, fmt=None):
         """FASTA/FASTQ(.gz) files -> kaiju output file, parsed / classified / formatted on the device (blocked gzip, BGZF, is inflated
-        there too; other gzip by zlib on the host).  Returns (reads, classified)."""
+        there too; other gzip by zlib on the host).  fmt: one of OUT_KAIJU (default), OUT_KAIJU_IDS (= verbose=True), OUT_KAIJU_V,
+        OUT_NAMES, OUT_NAMES_V (the last three need set_output_strings).  Returns (reads, classified lines)."""
+        if fmt is None:
+            fmt = OUT_KAIJU_IDS if verbose else OUT_KAIJU
         n = C.c_uint64(); k = C.c_uint64()
         _check(lib().kj_classify_files(self._ctx, in1.encode(), in2.encode() if in2 else None, out_path.encode() if out_path else None,
-                                       1 if verbose else 0, C.byref(n), C.byref(k)))
+                                       int(fmt), C.byref(n), C.byref(k)))
         return int(n.value), int(k.value)
+
+    def set_output_strings(self, kind, strings):
+        """The strings classify_files prints in place of numbers (kj_set_output_strings): kind STR_ACCESSION, strings[r] = accession of rank r
+        (fmi_accessions); kind STR_TAXON, strings[k] = label of the taxon of dense index k (compact_ids order, without the last entry)."""
+        strings = [s.encode() if isinstance(s, str) else bytes(s) for s in strings]
+        off = np.zeros(len(strings) + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([len(s) for s in strings], dtype=np.uint64) if strings else []
+        blob = np.frombuffer(b"".join(strings) or b"\0", dtype=np.uint8)
+        _check(lib().kj_set_output_strings(self._ctx, int(kind), blob.ctypes.data, off.ctypes.data, len(strings)))
 
     @property
     def files_device_inflated_bytes(self):

@@ -290,6 +290,7 @@ struct kj_ctx {
     KjTierBuf sa_tax, seq_tax, sa_acc, seq_acc;     // in HBM, or in the host tier of a kj_create_tiered context
     KjHostBuf rank_host; uint64_t nb_dev = 0;       // compact tiered layout: records [nb_dev, nb) in the host tier, records [0, nb_dev) in `rank`
     KjDevBuf row_tax;              // taxon per BWT row (kj_device_build_row_tax; empty: the kernels walk)
+    KjTierBuf out_str[2], out_off[2]; uint64_t out_n[2] = {0, 0}, out_bytes[2] = {0, 0}; bool out_have[2] = {false, false};   // kj_set_output_strings, by kind
     uint64_t index_bytes = 0, host_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;      // HBM and pinned host memory of the index
     // run state
     KjDevBuf counter, err, maxlen, quirk;
@@ -883,6 +884,33 @@ extern "C" uint64_t kj_kernel_launches(const kj_ctx* c) { return c ? c->launches
 extern "C" uint64_t kj_index_bytes(const kj_ctx* c) { return c ? c->index_bytes : 0; }
 extern "C" uint64_t kj_index_host_bytes(const kj_ctx* c) { return c ? c->host_bytes : 0; }
 extern "C" int kj_index_layout(const kj_ctx* c) { return c ? c->H.wide : -1; }
+// The string tables kj_classify_files prints (accessions of `kaiju -v`, the front-ends' sequence names): where sa_acc goes, i.e. in HBM or, when
+// the context has a host tier, in mapped pinned host memory (a name table of an nr-scale index is GBs; the format pass reads a few strings per read).
+extern "C" int kj_set_output_strings(kj_ctx* c, int kind, const char* blob, const uint64_t* off, uint64_t n) {
+    if (!c || !off || (kind != KJ_STR_ACCESSION && kind != KJ_STR_TAXON)) { kj_err() = "kj_set_output_strings: null argument or unknown kind"; return KJ_ERR_ARG; }
+    if (kind == KJ_STR_TAXON && n + 1 != c->n_counts) { kj_err() = "kj_set_output_strings: the taxon table needs kj_counts_size() - 1 = " + std::to_string(c->n_counts - 1) + " strings"; return KJ_ERR_ARG; }
+    for (uint64_t k = 0; k < n; k++) if (off[k + 1] < off[k]) { kj_err() = "kj_set_output_strings: offsets must not decrease"; return KJ_ERR_ARG; }
+    if (off[0] != 0 || (off[n] && !blob)) { kj_err() = "kj_set_output_strings: off[0] must be 0 and blob hold off[n] bytes"; return KJ_ERR_ARG; }
+    CK(cudaSetDevice(c->device)); CK(cudaDeviceSynchronize());       // no kernel reads the table being replaced
+    KjTierBuf& S = c->out_str[kind]; KjTierBuf& O = c->out_off[kind]; const bool host = c->sa_tax.on_host;
+    (S.on_host ? c->host_bytes : c->index_bytes) -= c->out_bytes[kind];
+    S.dev.reset(); S.host.reset(); O.dev.reset(); O.host.reset(); c->out_bytes[kind] = 0; c->out_n[kind] = 0; c->out_have[kind] = false;
+    S.on_host = O.on_host = host;
+    const size_t sb = std::max<size_t>((size_t)off[n], 16), ob = (size_t)(n + 1) * 8;
+    for (KjTierBuf* b : {&S, &O}) {
+        const size_t need = b == &S ? sb : ob;
+        if (b->grow(need) != KJ_OK) {
+            cudaGetLastError(); S.dev.reset(); S.host.reset();
+            char m[240]; snprintf(m, sizeof m, "kj_set_output_strings: could not allocate %zu bytes of %s for the %s table (%llu strings, %llu bytes of text)", need,
+                                  host ? "pinned host memory" : "device memory", kind == KJ_STR_ACCESSION ? "accession" : "taxon label", (unsigned long long)n, (unsigned long long)off[n]);
+            kj_err() = m; return KJ_ERR_NOMEM;
+        }
+    }
+    int rc; if ((off[n] && (rc = S.put(blob, (size_t)off[n]))) || (rc = O.put(off, ob))) return rc;
+    c->out_bytes[kind] = sb + ob; (host ? c->host_bytes : c->index_bytes) += sb + ob;
+    c->out_n[kind] = n; c->out_have[kind] = true;
+    return KJ_OK;
+}
 extern "C" double kj_last_kernel_ms(const kj_ctx* c) {
     if (!c) return 0.0;
     float ms = 0.f; if (cudaEventSynchronize(c->ev_b) != cudaSuccess) return 0.0;
