@@ -191,6 +191,10 @@ void ko_get_suffix(const ko_index *x, int64_t i, int *iseq, int64_t *pos) {
     while (c && (i & x->check)) { c = x->letters[i]; i = rank_(x, c, i); k++; }
     if (c) {
         int64_t e = (i >> x->chpt_exp) - ((int64_t)(x->nseq - 1) >> x->chpt_exp) - 1;
+        /* The last sampled row of an index whose nseq is a multiple of 2^chpt_exp and whose bwtlen is not has no entry: the header counts one sample
+         * less than kaiju-mkbwt writes (suffixArray.c:160 vs 206-216).  The reference decodes the bytes after its array there (heap
+         * contents, often a sequence number >= nseq); the device reads its guard entry, "no taxon".  The oracle does as the device. */
+        if (e >= x->ncheck) { *iseq = -1; *pos = -1; return; }
         const uint8_t *p = x->sa + e * x->nbytes; int64_t v = 0;
         for (int b = 0; b < x->nbytes; b++) v = (v << 8) + p[b];
         *iseq = (int)(v >> x->pbits); *pos = (v & x->mask) + k;
@@ -563,6 +567,7 @@ static void ids_from_si(const ko_index *x, const si_t *s, idset *ids, ko_counter
     for (int64_t k = s->start; k < s->start + s->len; k++) {
         if (ids->n > 20) break;
         int iseq = get_suffix_counted(x, k, ctr);
+        if (iseq < 0) continue;                                    /* the guard row (ko_get_suffix) */
         uint64_t id = x->seq_taxon[iseq];
         if (id == ULONG_MAX) continue;
         ids_insert(ids, id);

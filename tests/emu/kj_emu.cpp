@@ -164,11 +164,13 @@ void* kjemu_create(const char* fmi_path, const char* nodes_path, const kj_params
     kj_fmi_free(f); if (t) kj_nodes_free(t);
     if (kj_build_evalue_breaks(*p, c->H.db_length, c->evbreaks) != KJ_OK) { fprintf(stderr, "kjemu: %s\n", kj_last_error()); delete c; return nullptr; }
     KjDevIndex& D = c->D; KjHostIndex& H = c->H; memset(&D, 0, sizeof D);
+    // the guard entry the device appends (create_ctx): the last sampled row of a reference-built index may have no suffix-array entry
+    const size_t n_sa = H.sa_tax.size(); H.sa_tax.push_back(KJ_TAX_BAD); if (!H.sa_acc.empty()) H.sa_acc.push_back(0xffffffffu);
     D.rank = H.rank.data(); D.nb = H.nb; D.letters = H.letters.data(); D.bwtlen = H.bwtlen; D.alen = H.alen;
     for (int a = 0; a <= H.alen; a++) D.C[a] = H.C[a];
     for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
     D.sa_tax = H.sa_tax.data(); D.seq_tax = H.seq_tax.data(); D.sa_acc = H.sa_acc.empty() ? nullptr : H.sa_acc.data(); D.seq_acc = H.seq_acc.empty() ? nullptr : H.seq_acc.data(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
-    D.n_sa = H.sa_tax.size(); D.nseq = H.nseq;
+    D.n_sa = n_sa; D.nseq = H.nseq;
     D.tax_parent = H.tax_parent.data(); D.tax_depth = H.tax_depth.data(); D.tax_id = H.tax_id.data(); D.n_tax = (uint32_t)H.tax_id.size();
     D.lnfact = H.lnfact.data(); D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? (H.wide ? (const void*)H.kmer.data() : (const void*)H.kmer32.data()) : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = &H.tables; D.quirk_lo = H.quirk_lo; D.quirk_d = H.quirk_d; D.mono = (H.quirk_lo == ~0ull && !getenv("KJ_EMU_NOMONO")) ? 1 : 0;
     return c;

@@ -18,8 +18,6 @@ int kjemu_use_row_tax(void* h, int on) {
     std::lock_guard<std::mutex> lk(g_row_tax_mu);
     std::vector<uint32_t>& rt = g_row_tax[h];
     if (rt.empty()) {
-        // the guard entry the device appends (create_ctx): the last sampled row of a reference-built index has no suffix-array entry
-        c->H.sa_tax.push_back(KJ_TAX_BAD); c->D.sa_tax = c->H.sa_tax.data();
         rt.resize(c->H.bwtlen);
         for (uint64_t k = 0; k < c->H.bwtlen; k++) rt[k] = kj_row_taxon<uint32_t>(c->D, k);
     }

@@ -26,7 +26,7 @@ names = ["rounds", "round_steps", "lane_steps", "chains", "blocks", "lookaheads"
          "id_reads", "kept", "sa_waves", "sa_lf_steps", "sa_dep_steps", "lq_tops", "lq_slots"]
 for kw in (dict(mode="mem"), dict(mode="greedy")):
     P = make_params(**kw); kp = KjParams(**P); h = E.kjemu_create(fmi.encode(), nodes.encode(), C.byref(kp))
-    have_array = E.kjemu_use_row_tax(h, 1)          # built once here (it also appends the suffix array's guard entry, as the device does)
+    have_array = E.kjemu_use_row_tax(h, 1)          # built once here
     otax, obest = orc.classify_batch(P, s1, o1, s2, o2)
     for lookup in ("walk", "row_tax"):
         if lookup == "row_tax" and not have_array:
