@@ -119,7 +119,22 @@ int kj_create_scaled(kj_ctx **out, int device, const kj_params *params, const kj
  * (kj_create for copies = 1); indexes that fit in HBM are built exactly as there. */
 int kj_create_tiered(kj_ctx **out, int device, const kj_params *params, const kj_index_view *index, const kj_taxonomy_view *taxonomy,
                      uint32_t copies, uint64_t host_bytes);
-double kj_index_build_ms(const kj_ctx *ctx);      /* wall time of the index construction inside kj_create / kj_create_scaled / kj_create_tiered */
+/* kj_create_group: one index (the K-fold one for copies > 1, as kj_create_scaled) spread over the HBM of the n GPUs devices[0..n), for indexes
+ * larger than one GPU.  Writes n contexts to out[0..n), one per listed device (1 <= n <= 8; a device may be listed more than once), that share one
+ * copy of the index: its compact records are cut into n contiguous segments, segment g in the HBM of devices[g], and every context's kernels
+ * read all segments over peer access (NVLink), which kj_create_group enables for every pair of distinct listed devices (KJ_ERR_UNSUPPORTED,
+ * naming the pair, where a pair has none; peer access is never disabled).  The suffix-array taxon and accession arrays lie whole on one device
+ * each.  Every context has its own superblock and k-mer tables, taxonomy and run state, and is a normal context: every classify entry point,
+ * kj_set_params, kj_set_max_read_len, the counts, kj_set_output_strings and kj_classify_files work on it, and kj_classify_multi over the
+ * group's contexts shards one batch over all its GPUs.  The layout is always 4 (compact spread), whatever the index size; results are
+ * identical to those of the same index held by one GPU.  Placement is planned before any large allocation: replicas and 4 GB of headroom per
+ * context, the construction's buffers on devices[0] (where it runs), the suffix-array arrays where most room is left, and the records in
+ * proportion to the room left per device (a device listed twice shares it between its two segments).  A group too small fails with
+ * KJ_ERR_NOMEM, and kj_last_error() names the bytes needed and the bytes free on each device.  On any failure nothing stays allocated.  The
+ * index lives until the last of the n contexts is destroyed (kj_destroy, in any order). */
+int kj_create_group(kj_ctx **out, int n, const int *devices, const kj_params *params, const kj_index_view *index, const kj_taxonomy_view *taxonomy,
+                    uint32_t copies);
+double kj_index_build_ms(const kj_ctx *ctx);      /* wall time of the index construction inside kj_create / kj_create_scaled / kj_create_tiered / kj_create_group */
 /* Device-native index file (SURVEY.md 8f-4): kj_native_index_write() transcodes once (the .fmi + nodes.dmp views as for kj_create) and
  * stores the arrays exactly as they are uploaded (one-hot rank records, packed letters, taxon-reduced suffix array, re-indexed
  * taxonomy, k-mer table); kj_create_from_native() then needs one sequential read and the upload -- no transcode at load time.
@@ -261,11 +276,12 @@ int kj_check_errors(kj_ctx *ctx);
 /* --- introspection --- */
 const char *kj_last_error(void);                  /* thread-local text of the last failure          */
 uint64_t kj_kernel_launches(const kj_ctx *ctx);   /* number of kernels this context has launched    */
-uint64_t kj_index_bytes(const kj_ctx *ctx);       /* bytes of HBM held by the index                 */
+uint64_t kj_index_bytes(const kj_ctx *ctx);       /* bytes of HBM held by the index (a group context: on its own device -- its segment, the
+                                                     suffix-array arrays placed there, its replicas) */
 uint64_t kj_index_host_bytes(const kj_ctx *ctx);  /* bytes of pinned host memory held by the index (its host tier, kj_create_tiered; else 0) */
 /* Rank layout of the context's index: 0 narrow (< 2^32 rows, 5.25 B per row), 1 wide (64-bit intervals, 3.5 B per row plus 0.67 B of packed
  * letters), 2 compact (64-bit intervals, 1.003 B per row, letters included), 3 compact with its records split between HBM and host memory
- * (kj_create_tiered).  A 64-bit index is built wide when the wide construction fits in the HBM free at creation, else compact; when neither
+ * (kj_create_tiered), 4 compact with its records in segments over the HBM of a group of GPUs (kj_create_group).  A 64-bit index is built wide when the wide construction fits in the HBM free at creation, else compact; when neither
  * fits, kj_create / kj_create_scaled fail with KJ_ERR_NOMEM and kj_last_error() names the bytes needed and the bytes free (kj_create_tiered:
  * see there).  -1 for a null context. */
 int kj_index_layout(const kj_ctx *ctx);

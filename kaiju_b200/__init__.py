@@ -91,6 +91,8 @@ def lib():
         if hasattr(L, "kj_create_tiered"):
             L.kj_create_tiered.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(KjParams), C.POINTER(KjIndexView), C.POINTER(KjTaxonomyView), C.c_uint32, C.c_uint64]
             L.kj_index_host_bytes.restype = C.c_uint64; L.kj_index_host_bytes.argtypes = [C.c_void_p]
+        if hasattr(L, "kj_create_group"):
+            L.kj_create_group.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_int), C.POINTER(KjParams), C.POINTER(KjIndexView), C.POINTER(KjTaxonomyView), C.c_uint32]
         if hasattr(L, "kj_index_layout"):
             L.kj_index_layout.restype = C.c_int; L.kj_index_layout.argtypes = [C.c_void_p]
         L.kj_last_kernel_ms.restype = C.c_double; L.kj_last_kernel_ms.argtypes = [C.c_void_p]
@@ -207,6 +209,38 @@ def classify_multi(classifiers, seq1, off1, seq2=None, off2=None, want_best=True
     return (tax, best) if want_best else tax
 
 
+def create_group(fmi_path, nodes_path, devices, params=None, copies=1, max_read_len=None, **kw):
+    """One index spread over the HBM of the GPUs `devices` (kj_create_group: a device may be listed more than once; at most 8): a list of
+    Classifiers, one per listed device, that share the index (layout 4).  Each is a normal Classifier; classify_multi over the list shards one
+    batch over all of them.  The index lives until the last of them is closed.  copies > 1: the K-fold index, as Classifier(copies=)."""
+    L = lib(); devices = [int(d) for d in devices]; n = len(devices)
+    params = params if params is not None else make_params(**kw)
+    ctxs = (C.c_void_p * max(n, 1))(); devs = (C.c_int * max(n, 1))(*devices)
+    fmi = C.c_void_p(); nodes = C.c_void_p()
+    _check(L.kj_fmi_load(fmi_path.encode(), C.byref(fmi)))
+    try:
+        _check(L.kj_nodes_load(nodes_path.encode(), C.byref(nodes)))
+        try:
+            iv = KjIndexView(); tv = KjTaxonomyView()
+            L.kj_fmi_view(fmi, C.byref(iv)); L.kj_nodes_view(nodes, C.byref(tv))
+            _check(L.kj_create_group(ctxs, n, devs, C.byref(params), C.byref(iv), C.byref(tv), int(copies)))
+            bwtlen, nseq = int(iv.bwtlen) * int(copies), int(iv.nseq) * int(copies)
+        finally:
+            L.kj_nodes_free(nodes)
+    finally:
+        L.kj_fmi_free(fmi)
+    group = [Classifier._wrap(C.c_void_p(ctxs[g]), devices[g], params, bwtlen, nseq) for g in range(n)]
+    if max_read_len is not None:
+        try:
+            for clf in group:
+                clf.set_max_read_len(max_read_len)
+        except Exception:
+            for clf in group:
+                clf.close()
+            raise
+    return group
+
+
 class Classifier:
     """One GPU context: the .fmi index and nodes.dmp taxonomy resident in HBM + run parameters.
     `Classifier(native_path, None)` loads a device-native index file written by write_native_index()."""
@@ -251,6 +285,13 @@ class Classifier:
         finally:
             L.kj_fmi_free(fmi)
         self.device = device
+
+    @classmethod
+    def _wrap(cls, ctx, device, params, bwtlen, nseq):
+        """a Classifier around a context created elsewhere (create_group)"""
+        self = cls.__new__(cls)
+        self._ctx = ctx; self.device = device; self.params = params; self.bwtlen = bwtlen; self.nseq = nseq
+        return self
 
     def set_max_read_len(self, bases):
         """Longest mate admitted, in bases (protein reads: bases // 3 residues), from MAX_READ_LEN (the default) to MAX_LONG_READ_LEN
@@ -391,7 +432,8 @@ class Classifier:
 
     @property
     def layout(self):
-        """Rank layout of the index: 0 narrow, 1 wide, 2 compact, 3 compact with records in host memory (kj_index_layout)."""
+        """Rank layout of the index: 0 narrow, 1 wide, 2 compact, 3 compact with records in host memory, 4 compact spread over a group of GPUs
+        (create_group) (kj_index_layout)."""
         return int(lib().kj_index_layout(self._ctx))
 
     @property

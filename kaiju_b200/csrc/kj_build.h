@@ -186,13 +186,25 @@ static int kj_bld_upload(void* d, const void* h, size_t bytes) {
 // device's address space).  The build writes the host tier directly through the mapped pointer rather than staging it in HBM and copying: the
 // stores are posted PCIe writes of whole 16-byte words, each byte is written once, and no HBM is needed for a staging buffer -- HBM is exactly
 // what an index with a host tier lacks.
+// The output addressing is a policy, Out::rec(...) = where record b goes: KjBldOutTwo for the HBM / host-tier split (rec_out, rec_host, nb_dev),
+// KjBldOutSpread for the segments of a group (kj_create_group, the table `spread`), which the build on the group's first device stores straight
+// into the owning device's HBM over peer access -- the same direct stores as into the host tier, and no staging copy.  Both instances take every
+// parameter and each reads only its own, so the two-output instance compiles to the code it had before the policy.
 #define KJ_CSB_RECS (1u << (KJ_CSB_SHIFT - 7))
-static __device__ __forceinline__ uint64_t* kj_bld_crec(uint64_t* dev, uint64_t* host, uint64_t nb_dev, uint64_t b) {
-    return b < nb_dev ? dev + b * KJ_RANK_WORDS_COMPACT : host + (b - nb_dev) * KJ_RANK_WORDS_COMPACT;
-}
+struct KjBldOutTwo {
+    static __device__ __forceinline__ uint64_t* rec(uint64_t* dev, uint64_t* host, uint64_t nb_dev, const KjSpreadRef&, uint64_t b) {
+        return b < nb_dev ? dev + b * KJ_RANK_WORDS_COMPACT : host + (b - nb_dev) * KJ_RANK_WORDS_COMPACT;
+    }
+};
+struct KjBldOutSpread {
+    static __device__ __forceinline__ uint64_t* rec(uint64_t*, uint64_t*, uint64_t, const KjSpreadRef& s, uint64_t b) {
+        const uint32_t g = kj_spread_seg(s, b); return (uint64_t*)s.base[g] + (b - s.first[g]) * KJ_RANK_WORDS_COMPACT;
+    }
+};
+template <class Out>
 __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* __restrict__ bwt, const __grid_constant__ KjBuildLcode lc, uint64_t s0, uint64_t row0, uint64_t n,
                                                                   uint32_t rep, uint64_t nb, uint64_t* __restrict__ rec_out, uint64_t* __restrict__ rec_host, uint64_t nb_dev,
-                                                                  uint32_t* __restrict__ sb_tot) {
+                                                                  uint32_t* __restrict__ sb_tot, const __grid_constant__ KjSpreadRef spread) {
     __shared__ uint8_t lcs[256];
     __shared__ __align__(16) uint16_t cnt[KJ_CSB_RECS][KJ_MAX_ALEN];    // #c in the first half of each record, then the midpoint counts
     __shared__ uint8_t full[KJ_CSB_RECS][KJ_MAX_ALEN];                  // #c in each record
@@ -216,7 +228,7 @@ __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* 
             }
             pw[5 * h] = p0; pw[5 * h + 1] = p1; pw[5 * h + 2] = p2; pw[5 * h + 3] = p3; pw[5 * h + 4] = p4;
         }
-        ulonglong2* o = (ulonglong2*)kj_bld_crec(rec_out, rec_host, nb_dev, b);
+        ulonglong2* o = (ulonglong2*)Out::rec(rec_out, rec_host, nb_dev, spread, b);
         #pragma unroll
         for (int q = 0; q < 5; q++) o[q] = make_ulonglong2(pw[2 * q], pw[2 * q + 1]);
     }
@@ -230,7 +242,7 @@ __global__ void __launch_bounds__(KJ_BLD_THREADS) kj_bld_compact(const uint8_t* 
     for (uint32_t r = threadIdx.x; r < KJ_CSB_RECS; r += KJ_BLD_THREADS) {
         const uint64_t b = (s << (KJ_CSB_SHIFT - 7)) + r;
         if (b >= nb) break;
-        const ulonglong2* src = (const ulonglong2*)&cnt[r][0]; ulonglong2* o = (ulonglong2*)(kj_bld_crec(rec_out, rec_host, nb_dev, b) + KJ_CPT_COUNT_WORD);
+        const ulonglong2* src = (const ulonglong2*)&cnt[r][0]; ulonglong2* o = (ulonglong2*)(Out::rec(rec_out, rec_host, nb_dev, spread, b) + KJ_CPT_COUNT_WORD);
         #pragma unroll
         for (int q = 0; q < 3; q++) o[q] = src[q];
     }
@@ -255,8 +267,13 @@ static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBu
     const uint64_t CH = kj_compact_chunk_rows(), sb_per_chunk = CH >> KJ_CSB_SHIFT;
     int rc; KjDevBuf bwt, sbt, small;
     const uint64_t nd = c->nb_dev;                      // records [nd, nb) go to the host tier (kj_choose_layout)
-    if ((rc = c->rank.grow(nd * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->rank_host.grow((nb - nd) * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
-    tot += nd * KJ_RANK_WORDS_COMPACT * 8 + nsb * KJ_CSB_STRIDE * 8; c->host_bytes += (nb - nd) * KJ_RANK_WORDS_COMPACT * 8;
+    if (c->group) {                                     // the group's segments are allocated (kj_group_alloc) and counted per device already
+        if ((rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
+        tot += nsb * KJ_CSB_STRIDE * 8;
+    } else {
+        if ((rc = c->rank.grow(nd * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->rank_host.grow((nb - nd) * KJ_RANK_WORDS_COMPACT * 8)) || (rc = c->letters.grow(nsb * KJ_CSB_STRIDE * 8))) return rc;
+        tot += nd * KJ_RANK_WORDS_COMPACT * 8 + nsb * KJ_CSB_STRIDE * 8; c->host_bytes += (nb - nd) * KJ_RANK_WORDS_COMPACT * 8;
+    }
     if ((rc = sbt.grow(nsb * KJ_CSB_STRIDE * 4)) || (rc = small.grow(3 * KJ_MAX_ALEN * 8 + 64))) return rc;
     uint64_t* d_tot = small.as<uint64_t>(); uint64_t* d_C = d_tot + KJ_MAX_ALEN + 1;
     if (rep == 1) { if ((rc = bwt.grow((size_t)std::min(CH, n)))) return rc; }
@@ -264,7 +281,8 @@ static int kj_device_build_compact(kj_ctx* c, const kj_index_view& v, const KjBu
     for (uint64_t s0 = 0; s0 < nsb; s0 += sb_per_chunk) {
         const uint64_t row0 = s0 << KJ_CSB_SHIFT, nsc = std::min(sb_per_chunk, nsb - s0);
         if (rep == 1 && row0 < n) CK(cudaMemcpy(bwt.p, v.bwt + row0, (size_t)(std::min(n, row0 + CH) - row0), cudaMemcpyHostToDevice));
-        kj_bld_compact<<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, c->rank.as<uint64_t>(), c->rank_host.as<uint64_t>(), nd, sbt.as<uint32_t>());
+        if (c->group) kj_bld_compact<KjBldOutSpread><<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, nullptr, nullptr, 0, sbt.as<uint32_t>(), c->group->ref);
+        else kj_bld_compact<KjBldOutTwo><<<(unsigned)nsc, KJ_BLD_THREADS>>>(bwt.as<uint8_t>(), lc, s0, row0, n, rep, nb, c->rank.as<uint64_t>(), c->rank_host.as<uint64_t>(), nd, sbt.as<uint32_t>(), KjSpreadRef{});
         CK(cudaGetLastError()); c->launches++;
         if (rep == 1) CK(cudaDeviceSynchronize());          // the next chunk's upload overwrites the staging buffer
     }
@@ -346,6 +364,97 @@ static int kj_choose_layout(kj_ctx* c, const kj_index_view& v, uint32_t rep, uin
     return KJ_OK;
 }
 
+// Placement of a compact spread index (kj_create_group) over the group's contexts cs[0..n) (cs[0] holds the meta data), before anything large is
+// allocated.  It starts from the HBM free on each distinct device (a device listed twice shares its free memory between its two segments) and
+// reserves, in this order:
+//   1. on each context's device: its replicas (superblock table, k-mer table, taxonomy and tables, counts) and KJ_TIER_HEADROOM for classifying;
+//   2. on the first device: the largest transient buffer of the construction (BWT chunk + superblock totals, suffix-array upload chunk, the second
+//      k-mer level buffer), which runs there;
+//   3. the suffix-array arrays (sa_tax, sa_acc, seq_tax, seq_acc), each whole on the device with the most room left;
+//   4. the records, cut into contiguous segments in group order, in proportion to the room each group member has left.
+// KJ_ERR_NOMEM when the group is too small; the message names the bytes needed and the bytes free on each device.  KJ_SPREAD_RECORDS=n0,n1,...
+// (developer hook) forces the record count of every segment but the last, which takes the rest.
+static int kj_plan_group(kj_ctx* const* cs, int n, const kj_index_view& v, uint32_t rep, KjGroup& G) {
+    kj_ctx* c0 = cs[0]; KjHostIndex& H = c0->H;
+    const uint64_t rows = H.bwtlen, nb = rows / KJ_RANK_ROWS_COMPACT + 1, nsb = kj_csb_count(rows), rec = KJ_RANK_WORDS_COMPACT * 8;
+    if (nb >= 0xffffffffull) { kj_err() = "kj_create_group: index of " + std::to_string(rows) + " rows has more than 2^32 - 2 compact records"; return KJ_ERR_UNSUPPORTED; }
+    H.wide = KJ_LAYOUT_COMPACT_SPREAD; H.nb = nb; c0->nb_dev = nb;
+    // free HBM per distinct device
+    std::vector<int> devs; std::vector<uint64_t> fr;
+    for (int g = 0; g < n; g++) {
+        if (std::find(devs.begin(), devs.end(), cs[g]->device) != devs.end()) continue;
+        KjDevGuard d(cs[g]->device); size_t f = 0, t = 0; CK(cudaMemGetInfo(&f, &t));
+        devs.push_back(cs[g]->device); fr.push_back(f);
+    }
+    auto slot = [&](int dev) { return (size_t)(std::find(devs.begin(), devs.end(), dev) - devs.begin()); };
+    std::vector<int64_t> room(fr.begin(), fr.end());
+    // 1. replicas + headroom per context
+    uint64_t kmer = 0;
+    { const char* ek = getenv("KJ_KMER_K"); const int k = ek ? atoi(ek) : kj_default_kmer_k(rows);
+      if (k >= 2 && k <= 7 && H.alen == 21) { kmer = sizeof(KjKmer); for (int d = 0; d < k; d++) kmer *= 20; } }
+    const uint64_t csb = nsb * KJ_CSB_STRIDE * 8, small = H.tax_parent.size() * 4 + H.tax_depth.size() * 4 + H.tax_id.size() * 8 + H.lnfact.size() * 8 +
+                         sizeof(KjTables) + (H.tax_id.size() + 1) * 16 + 4096;
+    const uint64_t replica = csb + kmer + small + KJ_TIER_HEADROOM;
+    for (int g = 0; g < n; g++) room[slot(cs[g]->device)] -= (int64_t)replica;
+    // 2. the construction's largest transient buffer, on the first device
+    const uint64_t n_sa = rep == 1 ? (uint64_t)v.ncheck + 1 : (uint64_t)std::max<int64_t>((int64_t)((rows - 1) >> H.sa_exp) - H.sa_bias + 1, 4);
+    const uint64_t upload = rep == 1 ? std::min<uint64_t>(1ull << 26, n_sa) * (uint64_t)v.nbytes : 0;
+    const uint64_t transient = std::max(std::max(nsb * KJ_CSB_STRIDE * 4 + (rep == 1 ? std::min(kj_compact_chunk_rows(), rows) : (uint64_t)v.bwtlen), upload), kmer);
+    room[slot(c0->device)] -= (int64_t)transient;
+    // 3. the suffix-array arrays, whole, each on the device with the most room left
+    const bool acc = !H.seq_acc.empty();
+    const uint64_t sa_bytes = std::max<uint64_t>(n_sa * 4 + 4, 16), seq_bytes = std::max<uint64_t>((uint64_t)H.nseq * 4, 16);
+    struct { KjTierBuf* b; uint64_t bytes; } arrays[4] = {{&c0->sa_tax, sa_bytes}, {&c0->sa_acc, acc ? sa_bytes : 0}, {&c0->seq_tax, seq_bytes}, {&c0->seq_acc, acc ? seq_bytes : 0}};
+    uint64_t sa_total = 0;
+    for (auto& a : arrays) {
+        if (!a.bytes) continue;
+        const size_t best = (size_t)(std::max_element(room.begin(), room.end()) - room.begin());
+        a.b->device = devs[best]; room[best] -= (int64_t)a.bytes; sa_total += a.bytes;
+    }
+    // 4. the records, in proportion to the room left per group member
+    std::vector<uint64_t> share((size_t)n, 0); unsigned __int128 total_share = 0; bool fits = true;
+    for (size_t d = 0; d < devs.size(); d++) if (room[d] < 0) fits = false;
+    for (int g = 0; g < n; g++) {
+        const size_t d = slot(cs[g]->device); const int64_t members = (int64_t)std::count_if(cs, cs + n, [&](const kj_ctx* x) { return x->device == devs[d]; });
+        share[(size_t)g] = room[d] > 0 ? (uint64_t)(room[d] / members) : 0; total_share += share[(size_t)g];
+    }
+    const char* hook = getenv("KJ_SPREAD_RECORDS");
+    if (!hook && (!fits || total_share < (unsigned __int128)nb * rec)) {
+        uint64_t need = nb * rec + sa_total + replica * (uint64_t)n + transient;
+        std::string m = "index of " + std::to_string(rows) + " rows does not fit in the HBM of the group: it needs " + std::to_string(need) + " bytes (records " +
+                        std::to_string(nb * rec) + ", suffix-array arrays " + std::to_string(sa_total) + ", " + std::to_string(replica) + " per context for its replicas and " +
+                        std::to_string((uint64_t)KJ_TIER_HEADROOM) + " bytes of headroom, construction " + std::to_string(transient) + "); free:";
+        for (size_t d = 0; d < devs.size(); d++) m += (d ? ", device " : " device ") + std::to_string(devs[d]) + " " + std::to_string(fr[d]) + " bytes";
+        kj_err() = m; return KJ_ERR_NOMEM;
+    }
+    G.n = n; G.first[0] = 0;
+    if (hook) {
+        const char* p = hook;
+        for (int g = 0; g + 1 < n; g++) {
+            const uint64_t want = *p ? strtoull(p, (char**)&p, 10) : 0; if (*p == ',') p++;
+            G.first[g + 1] = std::min(nb, G.first[g] + want);
+        }
+    } else {
+        unsigned __int128 cum = 0;
+        for (int g = 0; g + 1 < n; g++) { cum += share[(size_t)g]; G.first[g + 1] = (uint64_t)((unsigned __int128)nb * cum / total_share); }
+    }
+    G.first[n] = nb;
+    for (int g = 0; g < n; g++) G.dev[g] = cs[g]->device;
+    return KJ_OK;
+}
+// The segments kj_plan_group laid out, each on its owner's device, and the segment table of the descriptors.
+static int kj_group_alloc(KjGroup& G) {
+    memset(&G.ref, 0, sizeof G.ref);
+    for (int g = 0; g < KJ_MAX_GROUP; g++) G.ref.first[g] = ~0ull;
+    for (int g = 0; g < G.n; g++) {
+        KjDevGuard d(G.dev[g]);
+        int rc = G.seg[g].grow((size_t)(G.first[g + 1] - G.first[g]) * KJ_RANK_WORDS_COMPACT * 8); if (rc) return rc;
+        G.ref.base[g] = G.seg[g].as<const uint64_t>(); G.ref.first[g] = G.first[g];
+    }
+    G.ref.n = (uint32_t)G.n;
+    return KJ_OK;
+}
+
 // The one-hot layouts (narrow, wide): rank records and packed letters from the whole BWT on the device.
 static int kj_device_build_onehot(kj_ctx* c, const kj_index_view& v, const KjBuildLcode& lc, uint32_t rep, uint64_t& tot) {
     KjHostIndex& H = c->H; const int alen = H.alen; const uint64_t n = H.bwtlen, nb = H.nb; const int wide = H.wide;
@@ -423,7 +532,8 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
         const int64_t last = (int64_t)((n - 1) >> H.sa_exp) - H.sa_bias;  // entry of the last sampled row
         n_sa = last >= 0 ? (uint64_t)last + 1 : 0;
         if ((rc = tier_grow(c, c->sa_tax, std::max<size_t>(n_sa * 4, 16), tot))) return rc;
-        if (base->H.wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_sa_tax_scaled<KjTieredIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        if (base->H.wide == KJ_LAYOUT_COMPACT_SPREAD) kj_bld_sa_tax_scaled<KjSpreadIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
+        else if (base->H.wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_sa_tax_scaled<KjTieredIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else if (base->H.wide == KJ_LAYOUT_COMPACT) kj_bld_sa_tax_scaled<KjCompactIdx><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else if (base->H.wide) kj_bld_sa_tax_scaled<uint64_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
         else kj_bld_sa_tax_scaled<uint32_t><<<grid_big, 256>>>(base->ix.as<KjDevIndex>(), n_sa, H.sa_bias, H.sa_exp, n, rep, c->sa_tax.as<uint32_t>());
@@ -438,7 +548,8 @@ static int kj_device_build(kj_ctx* c, const kj_index_view& v, const uint8_t lcod
 static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, int& k_out) {
     KjHostIndex& H = c->H; const int wide = H.wide; const KjDevIndex* ix = c->ix.as<KjDevIndex>();
     if (H.quirk_lo != ~0ull && &dst == &c->kmer) {
-        if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_quirk<KjTieredIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        if (wide == KJ_LAYOUT_COMPACT_SPREAD) kj_bld_quirk<KjSpreadIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
+        else if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_quirk<KjTieredIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         else if (wide == KJ_LAYOUT_COMPACT) kj_bld_quirk<KjCompactIdx><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         else if (wide) kj_bld_quirk<uint64_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>()); else kj_bld_quirk<uint32_t><<<1, 32>>>(ix, H.bwtlen - 65536ull, c->quirk.as<uint64_t>());
         CK(cudaGetLastError()); CK(cudaMemcpy(H.quirk_d, c->quirk.p, sizeof H.quirk_d, cudaMemcpyDeviceToHost)); c->launches++;
@@ -455,7 +566,8 @@ static int kj_device_build_kmer(kj_ctx* c, int k, uint64_t& tot, KjDevBuf& dst, 
     uint64_t n_cur = 20;
     for (int d = 1; d < k; d++) {
         const unsigned g = (unsigned)std::min<uint64_t>((n_cur * 20 + 255) / 256, (uint64_t)c->sm_count * 32);
-        if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_kmer_level<KjTieredIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        if (wide == KJ_LAYOUT_COMPACT_SPREAD) kj_bld_kmer_level<KjSpreadIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
+        else if (wide == KJ_LAYOUT_COMPACT_TIERED) kj_bld_kmer_level<KjTieredIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         else if (wide == KJ_LAYOUT_COMPACT) kj_bld_kmer_level<KjCompactIdx><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         else if (wide) kj_bld_kmer_level<uint64_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>()); else kj_bld_kmer_level<uint32_t><<<g, 256>>>(ix, a.as<KjKmer>(), n_cur, b.as<KjKmer>());
         CK(cudaGetLastError()); c->launches++;

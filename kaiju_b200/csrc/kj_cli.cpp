@@ -24,6 +24,7 @@
 
 static uint32_t g_max_read_len = KJ_MAX_READ_LEN;      // -L: longest mate admitted (kj_set_max_read_len)
 static uint64_t g_host_bytes = 0;                      // -H: pinned host memory the index may take when it does not fit in HBM (kj_create_tiered)
+static bool g_pool = false;                            // -P: one index spread over the HBM of the -d devices (kj_create_group)
 static void die(const std::string& m) { fprintf(stderr, "Error: %s\n\n", m.c_str()); exit(EXIT_FAILURE); }
 static void usage(const char* prog) {
     fprintf(stderr, "kaiju-b200 (H100-native classification path of Kaiju)\n\nUsage:\n   %s -t nodes.dmp -f kaiju_db.fmi -i reads.fastq [-j reads2.fastq]\n\n"
@@ -32,18 +33,20 @@ static void usage(const char* prog) {
                     "   -z INT        accepted for compatibility (ignored: the GPU replaces the worker threads)\n   -a STRING     Run mode, either \"mem\"  or \"greedy\" (default: greedy)\n"
                     "   -e INT        Number of mismatches allowed in Greedy mode (default: 3)\n   -m INT        Minimum match length (default: 11)\n   -s INT        Minimum match score in Greedy mode (default: 65)\n"
                     "   -E FLOAT      Minimum E-value in Greedy mode (default: 0.01)\n   -x            Enable SEG low complexity filter (enabled by default)\n   -X            Disable SEG low complexity filter\n"
-                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -H GB         Pinned host memory (GiB) the index may take when it does not fit in GPU memory (default 0: GPU memory only); the part\n                 in host memory is read over PCIe, the results are the same\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences;\n                 with -M the matched fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  With several devices the data sets of the\n                 -i/-j/-o lists are classified in parallel, one context (index replica) per device\n", prog);
+                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -H GB         Pinned host memory (GiB) the index may take when it does not fit in GPU memory (default 0: GPU memory only); the part\n                 in host memory is read over PCIe, the results are the same\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences;\n                 with -M the matched fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  With several devices the data sets of the\n                 -i/-j/-o lists are classified in parallel, one context (index replica) per device\n"
+                    "   -P            Pool the GPU memory of the -d devices: one index spread over all of them (for indexes larger than one GPU; the devices\n                 read each other's memory over NVLink) instead of one replica per device; the data sets are handed out as without -P.\n                 Not with -H, -w, -M or a device-native index file\n", prog);
     exit(EXIT_FAILURE);
 }
 
 int main(int argc, char** argv) {
     kj_params P; P.mode = 1; P.min_fragment_length = 11; P.mismatches = 3; P.min_score = 65; P.seed_length = 7; P.use_evalue = 1; P.min_evalue = 0.01; P.seg = 1; P.input_is_protein = 0; P.name_mode = 0;
     std::string nodes_fn, fmi_fn, in1, in2, out_fn, native_out, table_fn, table_rank = "species", names_fn; bool verbose = false; std::string device_arg = "0", frontend; int c;
-    while ((c = getopt(argc, argv, "a:hd:pxXvn:m:e:E:l:t:f:i:j:s:z:o:w:T:r:N:M:L:H:")) != -1) {
+    while ((c = getopt(argc, argv, "a:hd:pxXvn:m:e:E:l:t:f:i:j:s:z:o:w:T:r:N:M:L:H:P")) != -1) {
         switch (c) {
             case 'a': if (!strcmp(optarg, "mem")) { P.mode = 0; P.use_evalue = 0; } else if (!strcmp(optarg, "greedy")) P.mode = 1; else { fprintf(stderr, "-a must be a valid mode.\n"); usage(argv[0]); } break;
             case 'h': usage(argv[0]); break;
             case 'd': device_arg = optarg; break;
+            case 'P': g_pool = true; break;
             case 'v': verbose = true; break;
             case 'p': P.input_is_protein = 1; break;
             case 'x': P.seg = 1; break;
@@ -73,6 +76,11 @@ int main(int argc, char** argv) {
     if (fmi_fn.empty()) { fprintf(stderr, "Error: Please specify the location of the FMI file, using the -f option.\n\n"); usage(argv[0]); }
     { const char* b = strrchr(argv[0], '/'); const std::string prog = b ? b + 1 : argv[0]; if (frontend.empty() && (prog == "kaijux" || prog == "kaijup")) frontend = prog; }
     const bool names = !frontend.empty();
+    if (g_pool) {       // a spread index is built from the reference's .fmi, over HBM alone, for the taxon path
+        if (g_host_bytes) die("-P cannot be combined with -H: a pooled index lives in GPU memory only.");
+        if (!native_out.empty()) die("-P cannot be combined with -w.");
+        if (names) die("-P cannot be combined with -M.");
+    }
     if (names) {      // -M kaijux | kaijup (or invoked under that name): report the names of the matching database sequences, no taxonomy
         if (frontend != "kaijux" && frontend != "kaijup") die("-M must be kaijux or kaijup");
         if (frontend == "kaijup" && !in2.empty()) die("kaijup takes one input file");
@@ -83,6 +91,7 @@ int main(int argc, char** argv) {
     // -f may name a device-native index file (written with -w): it holds the taxonomy too, so -t is not needed then
     bool native_in = false;
     { FILE* f = fopen(fmi_fn.c_str(), "rb"); char m[8] = {0}; if (f) { native_in = fread(m, 1, 8, f) == 8 && memcmp(m, "KJB200IX", 8) == 0; fclose(f); } }
+    if (g_pool && native_in) die("-P needs the reference's .fmi as -f (device-native index files hold no pooled layout)");
     if (names && native_in) die("-M needs the reference's .fmi as -f (a device-native index file holds no sequence names)");
     if (nodes_fn.empty() && !native_in && !names) { fprintf(stderr, "Error: Please specify the location of the nodes.dmp file, using the -t option.\n\n"); usage(argv[0]); }
     if (!native_out.empty()) {              // -w FILE: transcode .fmi + nodes.dmp into the device-native index file and exit (no GPU needed)
@@ -110,7 +119,8 @@ int main(int argc, char** argv) {
     if (device_arg == "all") { const int nd = kj_device_count(); if (nd <= 0) die("no CUDA device available (this program has no CPU fallback)"); for (int d = 0; d < nd; d++) devices.push_back(d); }
     else for (const std::string& t : split(device_arg)) devices.push_back(atoi(t.c_str()));
     if (devices.empty()) devices.push_back(0);
-    if (devices.size() > l1.size()) devices.resize(l1.size());                                           // no more contexts than data sets
+    if (!g_pool && devices.size() > l1.size()) devices.resize(l1.size());                                 // no more contexts than data sets (-P: every device holds part of the index)
+    if (g_pool && devices.size() > 8) die("-P pools at most 8 devices.");
     if (!table_fn.empty() && (names_fn.empty() || nodes_fn.empty())) die("The summary table (-T) needs names.dmp (-N) and nodes.dmp (-t).");
 
     kj_fmi* fmi = nullptr; kj_nodes* nodes = nullptr; kj_index_view iv; kj_taxonomy_view tv;
@@ -126,7 +136,11 @@ int main(int argc, char** argv) {
         } else kj_nodes_view(nodes, &tv);
     }
     std::vector<kj_ctx*> ctxs(devices.size(), nullptr);
-    {
+    if (g_pool) {       // one spread index, one context per device; the contexts take the data sets as replicas do
+        int rc = kj_create_group(ctxs.data(), (int)devices.size(), devices.data(), &P, &iv, &tv, 1);
+        for (size_t d = 0; rc == KJ_OK && d < ctxs.size(); d++) rc = kj_set_max_read_len(ctxs[d], g_max_read_len);
+        if (rc != KJ_OK) die(kj_last_error());
+    } else {
         std::vector<std::thread> th; std::mutex mu; std::string err;
         for (size_t d = 0; d < devices.size(); d++) th.emplace_back([&, d] {
             int rc = native_in ? kj_create_from_native(&ctxs[d], devices[d], &P, fmi_fn.c_str()) : kj_create_tiered(&ctxs[d], devices[d], &P, &iv, &tv, 1, g_host_bytes);

@@ -161,6 +161,23 @@ template <class IdxT> struct KjIsTiered { static constexpr bool v = false; };
 template <> struct KjIsTiered<KjTieredIdx> { static constexpr bool v = true; };
 static_assert(sizeof(KjTieredIdx) == 8 && !KjIsTiered<uint64_t>::v && !KjIsTiered<KjCompactIdx>::v && !KjIsCompact<KjTieredIdx>::v,
               "KjTieredIdx must be a 64-bit type distinct from uint64_t and KjCompactIdx");
+// The compact spread layout (records in segments over the HBM of a group of GPUs) runs them with IdxT = KjSpreadIdx: a fourth 64-bit type, built
+// like KjTieredIdx.
+struct KjSpreadIdx {
+    unsigned long long v;
+    KjSpreadIdx() = default;
+    KJ_HD constexpr KjSpreadIdx(unsigned long long x) : v(x) {}
+    KJ_HD constexpr operator unsigned long long() const { return v; }
+    KJ_HD KjSpreadIdx& operator-=(KjSpreadIdx d) { v -= d.v; return *this; }
+};
+template <class IdxT> struct KjIsSpread { static constexpr bool v = false; };
+template <> struct KjIsSpread<KjSpreadIdx> { static constexpr bool v = true; };
+static_assert(sizeof(KjSpreadIdx) == 8 && !KjIsSpread<uint64_t>::v && !KjIsSpread<KjCompactIdx>::v && !KjIsSpread<KjTieredIdx>::v &&
+              !KjIsCompact<KjSpreadIdx>::v && !KjIsTiered<KjSpreadIdx>::v, "KjSpreadIdx must be a 64-bit type distinct from the other index types");
+// where kj_crec finds a compact record: one array, two tiers, or the segments of a group
+#define KJ_CREC_ONE 0
+#define KJ_CREC_TIER 1
+#define KJ_CREC_SPREAD 2
 // compact layout: rank of letter c at row k from the plane words of k's half-record `pl` (5 independent loads, issued by the caller) plus the
 // midpoint count and the superblock count -- every address a function of (c, k) only, and no branch on the data
 static KJ_DEV uint64_t kj_crank_planes(const KjDevIndex& ix, const uint64_t* rec, const uint64_t pw[5], uint32_t c, uint64_t k) {
@@ -176,14 +193,26 @@ static KJ_DEV uint64_t kj_crank_planes(const KjDevIndex& ix, const uint64_t* rec
     const uint64_t v = sb + ((cw >> (16u * (c & 3u))) & 0xffffull);
     return h ? v + pc : v - pc;
 }
-// TIER = true (compact tiered layout): the record lies in HBM below the split, in mapped host memory above it -- the base and the index are
-// selected, not branched on, so the load addresses still follow from (c, k) alone
-template <bool TIER = false>
+// WHERE = KJ_CREC_TIER (compact tiered layout): the record lies in HBM below the split, in mapped host memory above it -- the base and the index
+// are selected, not branched on, so the load addresses still follow from (c, k) alone.  KJ_CREC_SPREAD (compact spread layout): the segment of
+// b = k >> 7 is the number of segment starts first[1..7] at or below b (an unrolled compare, unused slots hold ~0), then its base and first
+// record are selected by that number -- again no branch, and an empty segment is never chosen (the next one starts at the same record).
+// the segment of record b: record numbers are below 2^32 - 1 (kj_plan_group), so the compares take the low words (unused slots: 0xffffffff)
+static KJ_DEV uint32_t kj_spread_seg(const KjSpreadRef& s, uint64_t b) {
+    const uint32_t r = (uint32_t)b; uint32_t g = 0;
+    #pragma unroll
+    for (int i = 1; i < KJ_MAX_GROUP; i++) g += r >= (uint32_t)s.first[i] ? 1u : 0u;
+    return g;
+}
+template <int WHERE = KJ_CREC_ONE>
 static KJ_DEV const uint64_t* kj_crec(const KjDevIndex& ix, uint64_t k) {
-    if constexpr (TIER) {
+    if constexpr (WHERE == KJ_CREC_TIER) {
         const uint64_t b = k >> 7, nd = ix.tier.nb_dev; const bool dev = b < nd;
         const uint64_t* base = dev ? ix.rank : ix.tier.host;
         return base + (size_t)(dev ? b : b - nd) * KJ_RANK_WORDS_COMPACT;
+    } else if constexpr (WHERE == KJ_CREC_SPREAD) {
+        const uint64_t b = k >> 7; const uint32_t g = kj_spread_seg(ix.spread, b);
+        return ix.spread.base[g] + (size_t)(b - ix.spread.first[g]) * KJ_RANK_WORDS_COMPACT;
     } else return ix.rank + (size_t)(k >> 7) * KJ_RANK_WORDS_COMPACT;
 }
 static KJ_DEV void kj_cplanes(const uint64_t* rec, uint64_t k, uint64_t pw[5]) {
@@ -191,15 +220,15 @@ static KJ_DEV void kj_cplanes(const uint64_t* rec, uint64_t k, uint64_t pw[5]) {
     #pragma unroll
     for (int b = 0; b < 5; b++) pw[b] = kj_ld64(pl + b);
 }
-template <bool TIER = false>
+template <int WHERE = KJ_CREC_ONE>
 static KJ_DEV uint64_t kj_crank(const KjDevIndex& ix, uint32_t c, uint64_t k) {
-    const uint64_t* rec = kj_crec<TIER>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    const uint64_t* rec = kj_crec<WHERE>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
     return kj_crank_planes(ix, rec, pw, c, k);
 }
 // one LF step of the compact layout: the letter of row k and its rank, from k's record
-template <bool TIER = false>
+template <int WHERE = KJ_CREC_ONE>
 static KJ_DEV uint64_t kj_clf(const KjDevIndex& ix, uint64_t k, uint32_t& c) {
-    const uint64_t* rec = kj_crec<TIER>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
+    const uint64_t* rec = kj_crec<WHERE>(ix, k); uint64_t pw[5]; kj_cplanes(rec, k, pw);
     const uint32_t bit = (uint32_t)k & 63u; c = 0;
     #pragma unroll
     for (int b = 0; b < 5; b++) c |= (uint32_t)((pw[b] >> bit) & 1ull) << b;
@@ -209,7 +238,8 @@ static KJ_DEV const uint64_t* kj_letter_base(const KjDevIndex& ix, uint32_t c) {
 template <class IdxT>
 static KJ_DEV IdxT kj_rank(const KjDevIndex& ix, uint32_t c, IdxT k) {
     if constexpr (KjIsCompact<IdxT>::v) return (IdxT)kj_crank(ix, c, (uint64_t)k);
-    else if constexpr (KjIsTiered<IdxT>::v) return (IdxT)kj_crank<true>(ix, c, (uint64_t)k);
+    else if constexpr (KjIsTiered<IdxT>::v) return (IdxT)kj_crank<KJ_CREC_TIER>(ix, c, (uint64_t)k);
+    else if constexpr (KjIsSpread<IdxT>::v) return (IdxT)kj_crank<KJ_CREC_SPREAD>(ix, c, (uint64_t)k);
     else return kj_rank_at<IdxT>(kj_letter_base(ix, c), k);
 }
 // UpdateSI (bwt.c:160-173)
@@ -217,7 +247,8 @@ template <class IdxT>
 static KJ_DEV bool kj_update_si(const KjDevIndex& ix, uint32_t c, IdxT& lo, IdxT& hi) {
     IdxT nlo, nhi;
     if constexpr (KjIsCompact<IdxT>::v) { nlo = (IdxT)kj_crank(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank(ix, c, (uint64_t)hi); }
-    else if constexpr (KjIsTiered<IdxT>::v) { nlo = (IdxT)kj_crank<true>(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank<true>(ix, c, (uint64_t)hi); }
+    else if constexpr (KjIsTiered<IdxT>::v) { nlo = (IdxT)kj_crank<KJ_CREC_TIER>(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank<KJ_CREC_TIER>(ix, c, (uint64_t)hi); }
+    else if constexpr (KjIsSpread<IdxT>::v) { nlo = (IdxT)kj_crank<KJ_CREC_SPREAD>(ix, c, (uint64_t)lo); nhi = (IdxT)kj_crank<KJ_CREC_SPREAD>(ix, c, (uint64_t)hi); }
     else { const uint64_t* base = kj_letter_base(ix, c); nlo = kj_rank_at<IdxT>(base, lo); nhi = kj_rank_at<IdxT>(base, hi); }
     // the reference's checkpoint quirk (indexes with bwtlen = m * 2^16 only, kj_host.cpp): the last 129 positions rank lower by a per-letter
     // constant.  Such indexes are routed to the 64-bit kernels, so the 32-bit ones do not carry the test.
@@ -247,7 +278,8 @@ static KJ_DEV uint64_t kj_sa_locate(const KjDevIndex& ix, uint64_t k, bool& is_s
     KJ_ROLLED
     while (c != 0 && (k & ix.sa_check)) {
         if constexpr (KjIsCompact<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf(ix, k, c); if (q) k -= ix.quirk_d[c]; }
-        else if constexpr (KjIsTiered<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf<true>(ix, k, c); if (q) k -= ix.quirk_d[c]; }
+        else if constexpr (KjIsTiered<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf<KJ_CREC_TIER>(ix, k, c); if (q) k -= ix.quirk_d[c]; }
+        else if constexpr (KjIsSpread<IdxT>::v) { const bool q = k >= ix.quirk_lo; k = kj_clf<KJ_CREC_SPREAD>(ix, k, c); if (q) k -= ix.quirk_d[c]; }
         else { c = kj_letter(ix, k); const bool q = k >= ix.quirk_lo; k = (uint64_t)kj_rank<IdxT>(ix, c, (IdxT)k); if (q) k -= ix.quirk_d[c]; }
 #if defined(KJ_EMU)
         kj_emu_stats.sa_lf_steps++;

@@ -171,15 +171,17 @@ static KjKernel kj_select_kernel_t(bool gws, bool fixed, bool verbose, int role)
 }
 template <int MODE, class T>
 static KjKernel kj_select_long_kernel_t(bool verbose) { return verbose ? kj_classify_long_kernel<MODE, T, true> : kj_classify_long_kernel<MODE, T, false>; }
-// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact, 3 compact tiered (64-bit intervals; kj_layout.h).  long_reads: the batch holds mates longer than
+// layout: 0 narrow (32-bit intervals), 1 wide, 2 compact, 3 compact tiered, 4 compact spread (64-bit intervals; kj_layout.h).  long_reads: the batch holds mates longer than
 // KJ_MAX_READ_LEN (only the work space in global memory, the general profile and ROLE 0 exist for them).
 static KjKernel kj_select_kernel(int mode, int layout, bool gws, bool fixed, bool verbose, int role, bool long_reads = false) {
     if (long_reads) {
+        if (layout == KJ_LAYOUT_COMPACT_SPREAD) return mode == 0 ? kj_select_long_kernel_t<0, KjSpreadIdx>(verbose) : kj_select_long_kernel_t<1, KjSpreadIdx>(verbose);
         if (layout == KJ_LAYOUT_COMPACT_TIERED) return mode == 0 ? kj_select_long_kernel_t<0, KjTieredIdx>(verbose) : kj_select_long_kernel_t<1, KjTieredIdx>(verbose);
         if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_long_kernel_t<0, KjCompactIdx>(verbose) : kj_select_long_kernel_t<1, KjCompactIdx>(verbose);
         if (mode == 0) return layout ? kj_select_long_kernel_t<0, uint64_t>(verbose) : kj_select_long_kernel_t<0, uint32_t>(verbose);
         return layout ? kj_select_long_kernel_t<1, uint64_t>(verbose) : kj_select_long_kernel_t<1, uint32_t>(verbose);
     }
+    if (layout == KJ_LAYOUT_COMPACT_SPREAD) return mode == 0 ? kj_select_kernel_t<0, KjSpreadIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjSpreadIdx>(gws, fixed, verbose, role);
     if (layout == KJ_LAYOUT_COMPACT_TIERED) return mode == 0 ? kj_select_kernel_t<0, KjTieredIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjTieredIdx>(gws, fixed, verbose, role);
     if (layout == KJ_LAYOUT_COMPACT) return mode == 0 ? kj_select_kernel_t<0, KjCompactIdx>(gws, fixed, verbose, role) : kj_select_kernel_t<1, KjCompactIdx>(gws, fixed, verbose, role);
     if (mode == 0) return layout ? kj_select_kernel_t<0, uint64_t>(gws, fixed, verbose, role) : kj_select_kernel_t<0, uint32_t>(gws, fixed, verbose, role);
@@ -248,16 +250,42 @@ struct KjHostBuf {
     }
     template <class T> T* as() const { return (T*)d; }
 };
+// Makes `dev` the current device for its lifetime and restores the previous one (dev < 0: changes nothing).  The arrays of a group
+// (kj_create_group) are allocated, written and freed with the device that holds them current.
+struct KjDevGuard {
+    int prev = -1;
+    explicit KjDevGuard(int dev) { if (dev >= 0 && cudaGetDevice(&prev) == cudaSuccess && prev != dev) cudaSetDevice(dev); else prev = -1; }
+    ~KjDevGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    KjDevGuard(const KjDevGuard&) = delete; KjDevGuard& operator=(const KjDevGuard&) = delete;
+};
 // An index array the placement of kj_create_tiered may move to the host tier (kj_choose_layout sets on_host before it is allocated): in HBM or
-// in mapped pinned host memory, read by the kernels through `p` either way.
+// in mapped pinned host memory, read by the kernels through `p` either way.  device >= 0: in the HBM of that device (a suffix-array array of a
+// group, placed by kj_plan_group), read by the group's other devices over peer access.
 struct KjTierBuf {
-    KjDevBuf dev; KjHostBuf host; bool on_host = false; void* p = nullptr;
-    int grow(size_t need) { const int rc = on_host ? host.grow(need) : dev.grow(need); p = on_host ? host.d : dev.p; return rc; }
+    KjDevBuf dev; KjHostBuf host; bool on_host = false; void* p = nullptr; int device = -1;
+    int grow(size_t need) { KjDevGuard g(device); const int rc = on_host ? host.grow(need) : dev.grow(need); p = on_host ? host.d : dev.p; return rc; }
     template <class T> T* as() const { return (T*)p; }
     size_t cap() const { return on_host ? host.cap : dev.cap; }
     // bytes [off, off + n) = val; the host tier is written by the CPU (nothing on the device writes it at this point)
-    int fill(size_t off, int val, size_t n) { if (on_host) memset((char*)host.p + off, val, n); else CK(cudaMemset((char*)dev.p + off, val, n)); return KJ_OK; }
-    int put(const void* src, size_t n) { if (on_host) memcpy(host.p, src, n); else CK(cudaMemcpy(dev.p, src, n, cudaMemcpyHostToDevice)); return KJ_OK; }
+    int fill(size_t off, int val, size_t n) { KjDevGuard g(device); if (on_host) memset((char*)host.p + off, val, n); else CK(cudaMemset((char*)dev.p + off, val, n)); return KJ_OK; }
+    int put(const void* src, size_t n) { KjDevGuard g(device); if (on_host) memcpy(host.p, src, n); else CK(cudaMemcpy(dev.p, src, n, cudaMemcpyHostToDevice)); return KJ_OK; }
+    void reset() { KjDevGuard g(device); dev.reset(); host.reset(); p = nullptr; }
+};
+
+// The index a group of contexts shares (kj_create_group, layout 4): the record segments, each in the HBM of its group member's device, and the
+// suffix-array arrays, each whole on the device kj_plan_group chose.  Every context of the group holds a shared_ptr to it; the last kj_destroy
+// frees every array with its owning device current.
+struct KjGroup {
+    int n = 0; int dev[KJ_MAX_GROUP] = {0};         // group member g: its device, and segment g = records [first[g], first[g + 1]) in seg[g]
+    uint64_t first[KJ_MAX_GROUP + 1] = {0};
+    KjDevBuf seg[KJ_MAX_GROUP];
+    KjSpreadRef ref{};                              // the segment table of the descriptors (kj_group_alloc)
+    KjTierBuf sa_tax, seq_tax, sa_acc, seq_acc;     // moved here from the first context once the construction has written them
+    KjGroup() = default; KjGroup(const KjGroup&) = delete; KjGroup& operator=(const KjGroup&) = delete;
+    ~KjGroup() {
+        for (int g = 0; g < n; g++) { KjDevGuard d(dev[g]); seg[g].reset(); }
+        for (KjTierBuf* b : {&sa_tax, &seq_tax, &sa_acc, &seq_acc}) b->reset();
+    }
 };
 
 // One of the two pipeline slots (the chunks of kj_classify, the lanes of kj_classify_files): staging, outputs, scratch, streams.
@@ -289,6 +317,8 @@ struct kj_ctx {
     KjDevBuf rank, letters, tax_parent, tax_depth, tax_id, lnfact, kmer;    // compact layout: `letters` holds the superblock table
     KjTierBuf sa_tax, seq_tax, sa_acc, seq_acc;     // in HBM, or in the host tier of a kj_create_tiered context
     KjHostBuf rank_host; uint64_t nb_dev = 0;       // compact tiered layout: records [nb_dev, nb) in the host tier, records [0, nb_dev) in `rank`
+    std::shared_ptr<KjGroup> group;                 // compact spread layout: the records and suffix-array arrays the group shares (`rank` and the
+                                                    // suffix-array members above stay empty; the superblock and k-mer tables are this context's own)
     KjDevBuf row_tax;              // taxon per BWT row (kj_device_build_row_tax; empty: the kernels walk)
     KjTierBuf out_str[2], out_off[2]; uint64_t out_n[2] = {0, 0}, out_bytes[2] = {0, 0}; bool out_have[2] = {false, false};   // kj_set_output_strings, by kind
     uint64_t index_bytes = 0, host_bytes = 0; uint64_t n_sa = 0; double build_ms = 0.0;      // HBM and pinned host memory of the index
@@ -321,10 +351,12 @@ template <class T> static int upload(const std::vector<T>& v, KjDevBuf& d, uint6
     if (!v.empty()) CK(cudaMemcpy(d.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
     total += bytes; return KJ_OK;
 }
-// an array that may live in the host tier: its bytes count towards the context's host bytes there, towards `total` (HBM) otherwise
+// an array that may live in the host tier: its bytes count towards the context's host bytes there, towards `total` (HBM) otherwise (a group's
+// array, placed on a device of its own, is counted by create_group_device)
 static int tier_grow(kj_ctx* c, KjTierBuf& b, size_t bytes, uint64_t& total) {
     int rc = b.grow(bytes); if (rc) return rc;
-    (b.on_host ? c->host_bytes : total) += bytes; return KJ_OK;
+    if (b.device < 0) (b.on_host ? c->host_bytes : total) += bytes;
+    return KJ_OK;
 }
 template <class T> static int tier_upload(kj_ctx* c, const std::vector<T>& v, KjTierBuf& b, uint64_t& total) {
     int rc = tier_grow(c, b, std::max<size_t>(v.size() * sizeof(T), 16), total); if (rc) return rc;
@@ -396,8 +428,12 @@ static int upload_descriptor(kj_ctx* c) {
     for (int a = 0; a <= H.alen; a++) D.C[a] = H.C[a];
     if (!kj_is_compact(H.wide)) for (int a = 0; a < H.alen; a++) D.rank_base[a] = D.rank + (uint64_t)a * H.nb * kj_rank_words(H.wide);
     if (H.wide == KJ_LAYOUT_COMPACT_TIERED) { D.tier.host = c->rank_host.as<const uint64_t>(); D.tier.nb_dev = c->nb_dev; }
-    D.sa_acc = c->sa_acc.as<const uint32_t>(); D.seq_acc = c->seq_acc.as<const uint32_t>();
-    D.sa_tax = c->sa_tax.as<const uint32_t>(); D.seq_tax = c->seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
+    const KjGroup* G = c->group.get();
+    if (H.wide == KJ_LAYOUT_COMPACT_SPREAD) { D.spread = G->ref; D.rank = G->ref.base[0]; }
+    const KjTierBuf& sa_acc = G ? G->sa_acc : c->sa_acc; const KjTierBuf& seq_acc = G ? G->seq_acc : c->seq_acc;
+    const KjTierBuf& sa_tax = G ? G->sa_tax : c->sa_tax; const KjTierBuf& seq_tax = G ? G->seq_tax : c->seq_tax;
+    D.sa_acc = sa_acc.as<const uint32_t>(); D.seq_acc = seq_acc.as<const uint32_t>();
+    D.sa_tax = sa_tax.as<const uint32_t>(); D.seq_tax = seq_tax.as<const uint32_t>(); D.sa_check = H.sa_check; D.sa_exp = H.sa_exp; D.sa_bias = H.sa_bias;
     D.n_sa = c->n_sa; D.row_tax = c->row_tax.as<const uint32_t>(); D.nseq = H.nseq;
     D.tax_parent = c->tax_parent.as<const uint32_t>(); D.tax_depth = c->tax_depth.as<const uint32_t>(); D.tax_id = c->tax_id.as<const uint64_t>(); D.n_tax = (uint32_t)H.tax_id.size();
     D.lnfact = c->lnfact.as<const double>(); D.n_lnfact = (int)H.lnfact.size(); D.kmer = H.kmer_k ? c->kmer.p : nullptr; D.kmer_k = H.kmer_k; D.wide = H.wide; D.tables = c->tables.as<KjTables>();
@@ -508,6 +544,88 @@ extern "C" int kj_create_tiered(kj_ctx** out, int device, const kj_params* param
     if (host_bytes == 0) return kj_create_scaled(out, device, params, index, taxonomy, copies);
     return create_scaled(out, device, params, index, taxonomy, copies < 1 ? 1 : copies, host_bytes);
 }
+
+// Peer access between every ordered pair of distinct devices of a group: the kernels of each device read the record segments of the others.
+// Per-process CUDA context state; an access enabled before (by an earlier group) is kept, and none is ever disabled.
+static int kj_enable_peers(const int* devices, int n) {
+    for (int i = 0; i < n; i++)
+        for (int j = 0; j < n; j++) {
+            const int a = devices[i], b = devices[j];
+            if (a == b) continue;
+            int can = 0; CK(cudaDeviceCanAccessPeer(&can, a, b));
+            if (!can) { kj_err() = "kj_create_group: device " + std::to_string(a) + " has no peer access to device " + std::to_string(b) + " (its kernels could not read the records held there)"; return KJ_ERR_UNSUPPORTED; }
+            KjDevGuard d(a);
+            const cudaError_t e = cudaDeviceEnablePeerAccess(b, 0);
+            if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+            else if (e != cudaSuccess) { kj_err() = std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(e); return KJ_ERR_CUDA; }
+        }
+    return KJ_OK;
+}
+// kj_create_group: one compact spread index over the HBM of devices[0..n), one context per listed device.  The construction runs on the first
+// device (kj_plan_group, kj_group_alloc, kj_device_build: the records go straight into their owners' HBM); the first context's superblock and
+// k-mer tables are then copied peer to peer to the other contexts, which upload their own taxonomy, tables and run state.
+static int create_group_device(kj_ctx** out, int n, const int* devices, const kj_params* params, const kj_index_view& v, const kj_taxonomy_view& t, uint32_t copies) {
+    std::vector<std::unique_ptr<kj_ctx, void (*)(kj_ctx*)>> cs;      // every early return below releases all contexts, and with the last the group
+    std::vector<kj_ctx*> raw;
+    for (int g = 0; g < n; g++) {
+        kj_ctx* c = nullptr; int rc = new_ctx(&c, devices[g], params); if (rc) return rc;
+        cs.emplace_back(c, kj_destroy); raw.push_back(c);
+    }
+    int rc = kj_enable_peers(devices, n); if (rc) return rc;
+    auto G = std::make_shared<KjGroup>();
+    for (kj_ctx* c : raw) c->group = G;
+    kj_ctx* c0 = raw[0];
+    CK(cudaSetDevice(c0->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    // the scaled build resolves its suffix-array rows through a base context of the index on the first device (freed after the construction)
+    std::unique_ptr<kj_ctx, void (*)(kj_ctx*)> base(nullptr, kj_destroy);
+    if (copies > 1) {
+        kj_ctx* b = nullptr; kj_transient_ctx = true; rc = create_ctx_device(&b, c0->device, params, v, t, 1, nullptr, 0); kj_transient_ctx = false; if (rc) return rc;
+        base.reset(b); CK(cudaSetDevice(c0->device));
+    }
+    uint8_t lcode[256]; if ((rc = kj_build_host_meta(v, t, copies, c0->H, lcode))) return rc;
+    if ((rc = kj_plan_group(raw.data(), n, v, copies, *G)) || (rc = kj_group_alloc(*G))) return rc;
+    uint64_t tot = 0;
+    if ((rc = upload_small(c0, tot)) || (rc = kj_device_build(c0, v, lcode, copies, base.get(), tot))) return rc;
+    base.reset();
+    G->sa_tax = std::move(c0->sa_tax); G->seq_tax = std::move(c0->seq_tax); G->sa_acc = std::move(c0->sa_acc); G->seq_acc = std::move(c0->seq_acc);
+    c0->H.kmer_k = 0;
+    if ((rc = upload_descriptor(c0))) return rc;
+    { const char* ek = getenv("KJ_KMER_K"); if ((rc = kj_device_build_kmer(c0, ek ? atoi(ek) : kj_default_kmer_k(c0->H.bwtlen), tot, c0->kmer, c0->H.kmer_k))) return rc; }
+    std::vector<uint32_t>().swap(c0->H.seq_tax);
+    if ((rc = finish_ctx(c0, tot))) return rc;
+    // the other members: the first context's meta data, its superblock and k-mer tables (peer to peer), their own small arrays and run state
+    for (int g = 1; g < n; g++) {
+        kj_ctx* c = raw[g]; CK(cudaSetDevice(c->device));
+        c->H = c0->H; c->nb_dev = c0->nb_dev; c->n_sa = c0->n_sa; uint64_t ct = 0;
+        if ((rc = upload_small(c, ct)) || (rc = c->letters.grow(c0->letters.cap))) return rc;
+        CK(cudaMemcpyPeer(c->letters.p, c->device, c0->letters.p, c0->device, c0->letters.cap)); ct += c0->letters.cap;
+        if (c0->kmer.p) {
+            if ((rc = c->kmer.grow(c0->kmer.cap))) return rc;
+            CK(cudaMemcpyPeer(c->kmer.p, c->device, c0->kmer.p, c0->device, c0->kmer.cap)); ct += c0->kmer.cap;
+        }
+        if ((rc = finish_ctx(c, ct))) return rc;
+    }
+    // kj_index_bytes: each context's replicas, its segment, and the suffix-array arrays on its device (counted at the first context there)
+    for (int g = 0; g < n; g++) {
+        kj_ctx* c = raw[g]; c->index_bytes += G->seg[g].cap;
+        if (std::find(devices, devices + g, c->device) != devices + g) continue;
+        for (const KjTierBuf* b : {&G->sa_tax, &G->seq_tax, &G->sa_acc, &G->seq_acc}) if (b->p && b->device == c->device) c->index_bytes += b->cap();
+    }
+    for (kj_ctx* c : raw) { CK(cudaSetDevice(c->device)); CK(cudaDeviceSynchronize()); }
+    const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (int g = 0; g < n; g++) { raw[g]->build_ms = ms; out[g] = cs[g].release(); }
+    return KJ_OK;
+}
+extern "C" int kj_create_group(kj_ctx** out, int n, const int* devices, const kj_params* params, const kj_index_view* index, const kj_taxonomy_view* taxonomy, uint32_t copies) {
+    if (!out || !devices || !params || !index || !taxonomy) { kj_err() = "kj_create_group: null argument"; return KJ_ERR_ARG; }
+    if (n < 1 || n > KJ_MAX_GROUP) { kj_err() = "kj_create_group: a group has 1 to " + std::to_string(KJ_MAX_GROUP) + " devices, not " + std::to_string(n); return KJ_ERR_ARG; }
+    const int ndev = kj_device_count();
+    for (int g = 0; g < n; g++)
+        if (ndev > 0 && (devices[g] < 0 || devices[g] >= ndev)) { kj_err() = "kj_create_group: device ordinal " + std::to_string(devices[g]) + " out of range"; return KJ_ERR_ARG; }
+    for (int g = 0; g < n; g++) out[g] = nullptr;
+    return create_group_device(out, n, devices, params, *index, *taxonomy, copies < 1 ? 1 : copies);
+}
 extern "C" double kj_index_build_ms(const kj_ctx* c) { return c ? c->build_ms : 0.0; }
 // test hook: checksums of the index arrays as they sit in memory (rank, letters or the compact superblock table, sa_tax, seq_tax, kmer | bwtlen,
 // layout, n_sa), to compare the device construction with the host transcoder array for array.  The records of a compact tiered index are its
@@ -517,12 +635,18 @@ extern "C" int kj_debug_index_checksums(kj_ctx* c, uint64_t out[8]) {
     const KjHostIndex& H = c->H; memset(out, 0, 64);
     const size_t sz[5] = {(size_t)kj_rank_array_words(H.wide, H.alen, H.nb) * 8, (size_t)kj_letters_words(H.wide, H.bwtlen) * 8, (size_t)c->n_sa * 4, (size_t)H.nseq * 4,
                           H.kmer_k ? (size_t)pow(20.0, H.kmer_k) * (H.wide ? sizeof(KjKmer) : sizeof(KjKmer32)) : 0};
-    const void* ptr[5] = {c->rank.p, c->letters.p, c->sa_tax.p, c->seq_tax.p, c->kmer.p};
-    const size_t dev0 = H.wide == KJ_LAYOUT_COMPACT_TIERED ? (size_t)c->nb_dev * KJ_RANK_WORDS_COMPACT * 8 : sz[0];      // bytes of the records in HBM
+    const KjGroup* G = c->group.get();
+    const void* ptr[5] = {c->rank.p, c->letters.p, G ? G->sa_tax.p : c->sa_tax.p, G ? G->seq_tax.p : c->seq_tax.p, c->kmer.p};
+    const size_t dev0 = H.wide == KJ_LAYOUT_COMPACT_TIERED ? (size_t)c->nb_dev * KJ_RANK_WORDS_COMPACT * 8 : G ? 0 : sz[0];      // bytes of the records in `rank`
     for (int i = 0; i < 5; i++) {
         std::vector<uint8_t> h(sz[i]); const size_t nd = i == 0 ? dev0 : sz[i];
         if (nd) CK(cudaMemcpy(h.data(), ptr[i], nd, cudaMemcpyDefault));
-        if (i == 0 && sz[0] > dev0) memcpy(h.data() + dev0, c->rank_host.p, sz[0] - dev0);
+        if (i == 0 && G) {      // compact spread: the segments in group order
+            for (int g = 0; g < G->n; g++) {
+                const size_t o = (size_t)G->first[g] * KJ_RANK_WORDS_COMPACT * 8, b = (size_t)(G->first[g + 1] - G->first[g]) * KJ_RANK_WORDS_COMPACT * 8;
+                if (b) CK(cudaMemcpy(h.data() + o, G->seg[g].p, b, cudaMemcpyDefault));
+            }
+        } else if (i == 0 && sz[0] > dev0) memcpy(h.data() + dev0, c->rank_host.p, sz[0] - dev0);
         out[i] = kj_mix_bytes(0x6b616a75ull + i, h.data(), h.size());
     }
     out[5] = H.bwtlen; out[6] = (uint64_t)H.wide; out[7] = c->n_sa;
@@ -742,7 +866,7 @@ static int classify_host(kj_ctx* c, const char* seq1, const uint64_t* off1, cons
     uint64_t chunk_reads = KJ_CHUNK_READS;
     if (const char* v = getenv("KJ_CHUNK_READS")) { long x = atol(v); if (x >= 1024 && x <= (1 << 24)) chunk_reads = (uint64_t)x; }       // tuning hook
     if (o.acc || o.frag) {
-        if (o.acc && !c->sa_acc.p) { kj_err() = "kj_classify_verbose2: the context was created without kj_index_view.seq_accession"; return KJ_ERR_UNSUPPORTED; }
+        if (o.acc && !c->dix.sa_acc) { kj_err() = "kj_classify_verbose2: the context was created without kj_index_view.seq_accession"; return KJ_ERR_UNSUPPORTED; }
         if ((o.acc && !o.nacc) || (o.frag && (!o.fraglen || o.frag_stride < 16))) { kj_err() = "kj_classify_verbose2: null argument"; return KJ_ERR_ARG; }
     }
     // per-read arrays of both slots, for the largest chunk

@@ -950,7 +950,7 @@ extern "C" int kj_classify_files(kj_ctx* c, const char* in1, const char* in2, co
     if (format < KJ_OUT_KAIJU || format > KJ_OUT_NAMES_V) { kj_err() = "kj_classify_files: unknown output format " + std::to_string(format); return KJ_ERR_ARG; }
     if (format >= KJ_OUT_NAMES && !c->params.name_mode) { kj_err() = "kj_classify_files: the name formats (KJ_OUT_NAMES, KJ_OUT_NAMES_V) need a context in name_mode"; return KJ_ERR_ARG; }
     if (format >= KJ_OUT_NAMES && !c->out_have[KJ_STR_TAXON]) { kj_err() = "kj_classify_files: the name formats need the KJ_STR_TAXON table (kj_set_output_strings)"; return KJ_ERR_ARG; }
-    if (format == KJ_OUT_KAIJU_V && !c->sa_acc.p) { kj_err() = "kj_classify_files: KJ_OUT_KAIJU_V needs a context created with kj_index_view.seq_accession"; return KJ_ERR_ARG; }
+    if (format == KJ_OUT_KAIJU_V && !c->dix.sa_acc) { kj_err() = "kj_classify_files: KJ_OUT_KAIJU_V needs a context created with kj_index_view.seq_accession"; return KJ_ERR_ARG; }
     if (format == KJ_OUT_KAIJU_V && !c->out_have[KJ_STR_ACCESSION]) { kj_err() = "kj_classify_files: KJ_OUT_KAIJU_V needs the KJ_STR_ACCESSION table (kj_set_output_strings)"; return KJ_ERR_ARG; }
     if (c->params.input_is_protein && in2 && *in2) { kj_err() = "Protein input only supports one input file."; return KJ_ERR_ARG; }
     CK(cudaSetDevice(c->device));

@@ -36,11 +36,17 @@
 //   compact tiered (kj_create_tiered, indexes whose compact construction does not fit in HBM either): the compact records, split at record
 //          nb_dev: records [0, nb_dev) in HBM, records [nb_dev, nb) in pinned host memory mapped into the device's address space (read over PCIe).
 //          Everything else of the index stays in HBM.  The record format is the compact one; only the address of record b depends on the split.
-// Layout codes (KjDevIndex::wide, KjHostIndex::wide): 0 narrow, 1 wide, 2 compact, 3 compact tiered.
+//   compact spread (kj_create_group, indexes larger than the HBM of one GPU): the compact records cut into at most KJ_MAX_GROUP contiguous
+//          segments, segment g = records [first[g], first[g+1]) in the HBM of the group's g-th device, read by the kernels of every device of
+//          the group over peer access (NVLink).  Each device holds its own superblock table, k-mer table and taxonomy; the suffix-array arrays
+//          lie whole on one device each.  The record format is the compact one; only the address of record b depends on the segments.
+// Layout codes (KjDevIndex::wide, KjHostIndex::wide): 0 narrow, 1 wide, 2 compact, 3 compact tiered, 4 compact spread.
 #define KJ_LAYOUT_NARROW 0
 #define KJ_LAYOUT_WIDE 1
 #define KJ_LAYOUT_COMPACT 2
 #define KJ_LAYOUT_COMPACT_TIERED 3
+#define KJ_LAYOUT_COMPACT_SPREAD 4
+#define KJ_MAX_GROUP 8             // devices (and record segments) of a compact spread index
 #define KJ_RANK_ROWS_NARROW 64
 #define KJ_RANK_ROWS_WIDE 192
 #define KJ_RANK_ROWS_COMPACT 128
@@ -50,7 +56,7 @@
 #define KJ_CPT_COUNT_WORD 10       // compact record: the 16-bit midpoint counts start at word 10
 #define KJ_CSB_SHIFT 16            // compact superblock: 2^16 rows = 512 records
 #define KJ_CSB_STRIDE 24           // compact superblock table: words per superblock (KJ_MAX_ALEN)
-static inline bool kj_is_compact(int layout) { return layout == KJ_LAYOUT_COMPACT || layout == KJ_LAYOUT_COMPACT_TIERED; }     // the compact record format
+static inline bool kj_is_compact(int layout) { return layout == KJ_LAYOUT_COMPACT || layout == KJ_LAYOUT_COMPACT_TIERED || layout == KJ_LAYOUT_COMPACT_SPREAD; }     // the compact record format
 static inline uint32_t kj_rank_rows(int layout) { return kj_is_compact(layout) ? KJ_RANK_ROWS_COMPACT : layout ? KJ_RANK_ROWS_WIDE : KJ_RANK_ROWS_NARROW; }
 static inline uint32_t kj_rank_words(int layout) { return kj_is_compact(layout) ? KJ_RANK_WORDS_COMPACT : layout ? KJ_RANK_WORDS_WIDE : KJ_RANK_WORDS_NARROW; }
 // 64-bit words of the rank array: one record per (letter, block) in the one-hot layouts, one record per block in the compact one
@@ -87,13 +93,17 @@ struct KjTables {
 
 // compact tiered layout: records [nb_dev, nb) start at `host` (the device alias of mapped pinned host memory), record b at host + (b - nb_dev) * 16
 struct KjTierRef { const uint64_t* host; uint64_t nb_dev; };
+// compact spread layout: segment g holds records [first[g], first[g+1]) from base[g] on (a device address in the HBM of the group's g-th device);
+// first[] does not decrease, and the slots g >= n hold first[g] = ~0 (never selected) and base[g] = null
+struct KjSpreadRef { const uint64_t* base[KJ_MAX_GROUP]; uint64_t first[KJ_MAX_GROUP]; uint32_t n, pad; };
 // (the 32-bit members are paired so that the descriptor has no padding holes: the kernels stage it in shared memory next to the work spaces)
 struct KjDevIndex {
     const uint64_t* rank; uint64_t nb;          // [alen][nb] records of 2 (narrow) or 4 (wide) 64-bit words; compact: [nb] records of 16 words
-                                                // (compact tiered: records [0, tier.nb_dev) only)
+                                                // (compact tiered: records [0, tier.nb_dev) only; compact spread: segment 0)
     union {
         const uint64_t* rank_base[KJ_MAX_ALEN]; // narrow, wide: records of letter c (saves the multiply in the inner loop)
         KjTierRef tier;                         // compact tiered: where records [nb_dev, nb) are (the compact layouts do not use rank_base)
+        KjSpreadRef spread;                     // compact spread: the segment table
     };
     union {
         const uint64_t* letters;                // narrow, wide: the packed letters
@@ -108,7 +118,7 @@ struct KjDevIndex {
     const uint32_t* tax_parent; const uint32_t* tax_depth; const uint64_t* tax_id; uint32_t n_tax; int n_lnfact;
     const double* lnfact;
     const void* kmer; int kmer_k;               // direct-address table of k-mer intervals (KjKmer32 if !wide else KjKmer; 0 = off)
-    int wide;                                   // layout code: 0 narrow (32-bit interval kernels), 1 wide, 2 compact, 3 compact tiered (64-bit interval kernels)
+    int wide;                                   // layout code: 0 narrow (32-bit interval kernels), 1 wide, 2 compact, 3 compact tiered, 4 compact spread (64-bit interval kernels)
     int mono;                                   // 1: true FM index (match starts monotone in the end position); 0: the reference's checkpoint quirk applies (no chain bounds)
     uint64_t quirk_lo; const uint64_t* quirk_d;         // rows k >= quirk_lo: FMindex(c,k) -= quirk_d[c] (reference checkpoint quirk, ~0 = none; [KJ_MAX_ALEN] in global memory)
     const KjTables* tables;
@@ -117,6 +127,8 @@ struct KjDevIndex {
 // geometry of every kernel were derived from.
 static_assert(sizeof(KjTierRef) <= sizeof(const uint64_t*) * KJ_MAX_ALEN && sizeof(KjDevIndex) == 592 && offsetof(KjDevIndex, rank_base) == 16 &&
               offsetof(KjDevIndex, tier) == 16 && offsetof(KjDevIndex, letters) == 208 && offsetof(KjDevIndex, tables) == 584, "KjDevIndex layout changed");
+static_assert(sizeof(KjSpreadRef) == 136 && sizeof(KjSpreadRef) <= sizeof(const uint64_t*) * KJ_MAX_ALEN && offsetof(KjDevIndex, spread) == 16,
+              "the segment table must fit in rank_base's bytes");
 
 struct KjRunParams {
     int mode;                       // 0 MEM, 1 GREEDY
