@@ -226,6 +226,17 @@ int kj_device_count(void);                        /* number of usable CUDA devic
 #define KJ_OUT_NAMES_V 4      /* kaijux -v / kaijup -v: as 3 with the fragment strings after the last tab                   */
 int kj_classify_files(kj_ctx *ctx, const char *in1, const char *in2, const char *out_path, int format,
                       uint64_t *n_reads_out, uint64_t *n_classified_out);
+/* kj_classify_files over several contexts (1 to 8; replicas from kj_create / kj_create_tiered / kj_create_from_native, or the members of a
+ * kj_create_group; two contexts may share a device): one reader set and parser on ctxs[0]'s device; every context classifies whole batches on
+ * its own host thread, each batch on whichever context next has a free lane (contexts other than ctxs[0] copy the batch to their device with
+ * cudaMemcpyPeerAsync, which also works without peer access); the batches are written in input order.  The output file is byte-identical to
+ * what kj_classify_files(ctxs[0], ...) writes.  Each context adds the reads it classified to its own count vector (sum them); the two totals
+ * count all contexts; kj_files_device_inflated_bytes(ctxs[0]) reports the call.  KJ_ERR_ARG, before any file is opened: a null argument,
+ * n_ctx outside 1..8, a context listed twice, contexts that differ in kj_params, kj_set_max_read_len, the index (BWT length, sequence count,
+ * taxa), or a context that lacks what `format` needs.  The first error of any context wins, prefixed "device N: ".  n_ctx = 1 is
+ * kj_classify_files itself. */
+int kj_classify_files_multi(kj_ctx **ctxs, int n_ctx, const char *in1, const char *in2, const char *out_path, int format,
+                            uint64_t *n_reads_out, uint64_t *n_classified_out);
 /* The strings kj_classify_files prints in place of numbers: string k = blob[off[k], off[k + 1]), off has n + 1 entries.
  *   KJ_STR_ACCESSION: n = number of distinct accessions, string r = accession of rank r (kj_index_view.seq_accession, column 6 of -v)
  *   KJ_STR_TAXON:     n = kj_counts_size(ctx) - 1, string k = label printed for the taxon of dense index k (kj_counts_get order)

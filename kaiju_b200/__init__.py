@@ -97,6 +97,8 @@ def lib():
             L.kj_index_layout.restype = C.c_int; L.kj_index_layout.argtypes = [C.c_void_p]
         L.kj_last_kernel_ms.restype = C.c_double; L.kj_last_kernel_ms.argtypes = [C.c_void_p]
         L.kj_classify_files.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        if hasattr(L, "kj_classify_files_multi"):
+            L.kj_classify_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.kj_counts_reset.argtypes = [C.c_void_p]
         L.kj_counts_size.restype = C.c_uint64; L.kj_counts_size.argtypes = [C.c_void_p]
         L.kj_counts_device_ptr.restype = C.c_void_p; L.kj_counts_device_ptr.argtypes = [C.c_void_p]
@@ -207,6 +209,20 @@ def classify_multi(classifiers, seq1, off1, seq2=None, off2=None, want_best=True
     arr = (C.c_void_p * len(classifiers))(*[c._ctx for c in classifiers])
     _check(lib().kj_classify_multi(arr, len(classifiers), seq1.ctypes.data, off1.ctypes.data, p2, o2, n, tax.ctypes.data, best.ctypes.data if want_best else None))
     return (tax, best) if want_best else tax
+
+
+def classify_files_multi(classifiers, in1, in2=None, out_path=None, verbose=False, fmt=None):
+    """Classifier.classify_files over several Classifiers (same index and parameters; replicas or the members of create_group) in this
+    process: one parser on the first one's GPU, whole batches classified by every Classifier, the output in input order and byte for byte
+    what the first Classifier alone writes (kj_classify_files_multi).  Each Classifier counts the reads it classified (sum their counts()).
+    Returns (reads, classified lines) over all of them."""
+    if fmt is None:
+        fmt = OUT_KAIJU_IDS if verbose else OUT_KAIJU
+    n = C.c_uint64(); k = C.c_uint64()
+    arr = (C.c_void_p * max(len(classifiers), 1))(*[c._ctx for c in classifiers])
+    _check(lib().kj_classify_files_multi(arr, len(classifiers), in1.encode(), in2.encode() if in2 else None, out_path.encode() if out_path else None,
+                                         int(fmt), C.byref(n), C.byref(k)))
+    return int(n.value), int(k.value)
 
 
 def create_group(fmi_path, nodes_path, devices, params=None, copies=1, max_read_len=None, **kw):

@@ -33,8 +33,8 @@ static void usage(const char* prog) {
                     "   -z INT        accepted for compatibility (ignored: the GPU replaces the worker threads)\n   -a STRING     Run mode, either \"mem\"  or \"greedy\" (default: greedy)\n"
                     "   -e INT        Number of mismatches allowed in Greedy mode (default: 3)\n   -m INT        Minimum match length (default: 11)\n   -s INT        Minimum match score in Greedy mode (default: 65)\n"
                     "   -E FLOAT      Minimum E-value in Greedy mode (default: 0.01)\n   -x            Enable SEG low complexity filter (enabled by default)\n   -X            Disable SEG low complexity filter\n"
-                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -H GB         Pinned host memory (GiB) the index may take when it does not fit in GPU memory (default 0: GPU memory only); the part\n                 in host memory is read over PCIe, the results are the same\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences;\n                 with -M the matched fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  With several devices the data sets of the\n                 -i/-j/-o lists are classified in parallel, one context (index replica) per device\n"
-                    "   -P            Pool the GPU memory of the -d devices: one index spread over all of them (for indexes larger than one GPU; the devices\n                 read each other's memory over NVLink) instead of one replica per device; the data sets are handed out as without -P.\n                 Not with -H, -w, -M or a device-native index file\n", prog);
+                    "   -w FILENAME   Write the device-native index file for -t/-f and exit; such a file can then be given as -f (no -t needed, no transcode at start-up)\n   -T FILENAME   Also write kaiju2table's summary (reads per taxon of rank -r, default species; needs -N names.dmp) from the counts kept on the GPU\n   -p            Input sequences are protein sequences\n   -L INT        Longest read (bases per mate) to accept, 16383 to 1048575 (default 16383; protein reads: a third of it).  Reads above 16383 bases\n                 run on the long-read kernels, whose per-warp scratch grows with the read length\n   -H GB         Pinned host memory (GiB) the index may take when it does not fit in GPU memory (default 0: GPU memory only); the part\n                 in host memory is read over PCIe, the results are the same\n   -v            Enable verbose output (adds the match length/score, the matching taxon ids, accession numbers and fragment sequences;\n                 with -M the matched fragment sequences)\n   -M STRING     front-end: \"kaijux\" (as kaiju, but reports the names of the matching database sequences; no -t) or \"kaijup\" (the same for protein reads)\n   -d LIST       CUDA device ordinal(s): one number, a comma-separated list, or \"all\" (default 0).  One context (index replica) per listed device.  With at least as many\n                 data sets (-i/-j/-o lists) as devices, the data sets are classified in parallel, each on one device; with fewer, one after\n                 another, each split into batches over all devices (a device may be listed twice: two contexts on one card)\n"
+                    "   -P            Pool the GPU memory of the -d devices: one index spread over all of them (for indexes larger than one GPU; the devices\n                 read each other's memory over NVLink) instead of one replica per device; the data sets are classified as without -P.\n                 Not with -H, -w, -M or a device-native index file\n", prog);
     exit(EXIT_FAILURE);
 }
 
@@ -114,12 +114,13 @@ int main(int argc, char** argv) {
     if (!lo.empty() && lo.size() != l1.size()) die("Length of input and output file lists differ");
     if (lo.empty() && l1.size() > 1) die("Several input files need a list of output files (-o)");
 
-    // devices: one context (index replica) per device; the data sets of the lists are handed out to whichever device is free
+    // devices: one context (index replica) per listed device.  With at least as many data sets as contexts, each data set goes whole to whichever
+    // context is free; with fewer, the data sets run one after another, each one over all contexts (kj_classify_files_multi)
     std::vector<int> devices;
     if (device_arg == "all") { const int nd = kj_device_count(); if (nd <= 0) die("no CUDA device available (this program has no CPU fallback)"); for (int d = 0; d < nd; d++) devices.push_back(d); }
     else for (const std::string& t : split(device_arg)) devices.push_back(atoi(t.c_str()));
     if (devices.empty()) devices.push_back(0);
-    if (!g_pool && devices.size() > l1.size()) devices.resize(l1.size());                                 // no more contexts than data sets (-P: every device holds part of the index)
+    if (!g_pool && l1.size() < devices.size() && devices.size() > 8) devices.resize(8);      // one data set over several contexts: at most 8 (kj_classify_files_multi)
     if (g_pool && devices.size() > 8) die("-P pools at most 8 devices.");
     if (!table_fn.empty() && (names_fn.empty() || nodes_fn.empty())) die("The summary table (-T) needs names.dmp (-N) and nodes.dmp (-t).");
 
@@ -141,12 +142,20 @@ int main(int argc, char** argv) {
         for (size_t d = 0; rc == KJ_OK && d < ctxs.size(); d++) rc = kj_set_max_read_len(ctxs[d], g_max_read_len);
         if (rc != KJ_OK) die(kj_last_error());
     } else {
+        // one thread per distinct device; the contexts of one device are created one after another (the construction sizes its temporary
+        // buffers from the free HBM it finds, which a second construction running beside it would take away)
         std::vector<std::thread> th; std::mutex mu; std::string err;
-        for (size_t d = 0; d < devices.size(); d++) th.emplace_back([&, d] {
-            int rc = native_in ? kj_create_from_native(&ctxs[d], devices[d], &P, fmi_fn.c_str()) : kj_create_tiered(&ctxs[d], devices[d], &P, &iv, &tv, 1, g_host_bytes);
-            if (rc == KJ_OK) rc = kj_set_max_read_len(ctxs[d], g_max_read_len);
-            if (rc != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); }
-        });
+        for (size_t d = 0; d < devices.size(); d++) {
+            if (std::find(devices.begin(), devices.begin() + (long)d, devices[d]) != devices.begin() + (long)d) continue;
+            th.emplace_back([&, d] {
+                for (size_t e = d; e < devices.size(); e++) {
+                    if (devices[e] != devices[d]) continue;
+                    int rc = native_in ? kj_create_from_native(&ctxs[e], devices[e], &P, fmi_fn.c_str()) : kj_create_tiered(&ctxs[e], devices[e], &P, &iv, &tv, 1, g_host_bytes);
+                    if (rc == KJ_OK) rc = kj_set_max_read_len(ctxs[e], g_max_read_len);
+                    if (rc != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); return; }
+                }
+            });
+        }
         for (auto& x : th) x.join();
         if (!err.empty()) die(err);
     }
@@ -172,23 +181,39 @@ int main(int argc, char** argv) {
     // Comma-separated lists for -i / -j / -o process several data sets against the index loaded once per device (kaiju-multi.cpp:220-330).
     struct Done { uint64_t n_reads = 0, n_classified = 0, inflated = 0; double secs = 0; std::vector<uint64_t> ids, counts; };
     std::vector<Done> done(l1.size()); std::atomic<size_t> next(0); std::mutex mu; std::string err;
-    std::vector<std::thread> workers;
-    for (size_t d = 0; d < ctxs.size(); d++) workers.emplace_back([&, d] {
-        for (;;) {
-            const size_t k = next.fetch_add(1); if (k >= l1.size()) return;
-            { std::lock_guard<std::mutex> lk(mu); if (!err.empty()) return; }
-            Done& r = done[k]; kj_ctx* ctx = ctxs[d]; int rc = KJ_OK;
-            if (!table_fn.empty()) rc = kj_counts_reset(ctx);
-            const auto t0 = std::chrono::steady_clock::now();
-            if (rc == KJ_OK) rc = kj_classify_files(ctx, l1[k].c_str(), paired ? l2[k].c_str() : nullptr, lo.empty() ? nullptr : lo[k].c_str(), fmt, &r.n_reads, &r.n_classified);
-            r.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-            r.inflated = kj_files_device_inflated_bytes(ctx);
-            if (rc == KJ_OK && !table_fn.empty()) { r.ids.resize(kj_counts_size(ctx)); r.counts.resize(r.ids.size()); rc = kj_counts_get(ctx, r.ids.data(), r.counts.data()); }
-            if (rc != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); return; }
+    // data set k on the contexts cs[0, n): its output, and with -T the sum of the contexts' counts (their id lists are the same)
+    auto run_set = [&](size_t k, kj_ctx** cs, int n) -> int {
+        Done& r = done[k]; int rc = KJ_OK;
+        for (int i = 0; rc == KJ_OK && i < n && !table_fn.empty(); i++) rc = kj_counts_reset(cs[i]);
+        const auto t0 = std::chrono::steady_clock::now();
+        if (rc == KJ_OK) rc = kj_classify_files_multi(cs, n, l1[k].c_str(), paired ? l2[k].c_str() : nullptr, lo.empty() ? nullptr : lo[k].c_str(), fmt, &r.n_reads, &r.n_classified);
+        r.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        r.inflated = kj_files_device_inflated_bytes(cs[0]);
+        if (rc == KJ_OK && !table_fn.empty()) {
+            r.ids.resize(kj_counts_size(cs[0])); r.counts.assign(r.ids.size(), 0);
+            std::vector<uint64_t> ids(r.ids.size()), cnt(r.ids.size());
+            for (int i = 0; rc == KJ_OK && i < n; i++) {
+                if ((rc = kj_counts_get(cs[i], ids.data(), cnt.data())) != KJ_OK) break;      // (kj_classify_files_multi checked that the vectors have one size)
+                if (i == 0) r.ids = ids; else if (ids != r.ids) die("the contexts of -d count different taxa");
+                for (size_t t = 0; t < cnt.size(); t++) r.counts[t] += cnt[t];
+            }
         }
-    });
-    for (auto& x : workers) x.join();
-    if (!err.empty()) die(err);
+        return rc;
+    };
+    if (l1.size() < ctxs.size()) {        // fewer data sets than contexts: each one over every context, in list order
+        for (size_t k = 0; k < l1.size(); k++) if (run_set(k, ctxs.data(), (int)ctxs.size()) != KJ_OK) die(kj_last_error());
+    } else {
+        std::vector<std::thread> workers;
+        for (size_t d = 0; d < ctxs.size(); d++) workers.emplace_back([&, d] {
+            for (;;) {
+                const size_t k = next.fetch_add(1); if (k >= l1.size()) return;
+                { std::lock_guard<std::mutex> lk(mu); if (!err.empty()) return; }
+                if (run_set(k, &ctxs[d], 1) != KJ_OK) { std::lock_guard<std::mutex> lk(mu); if (err.empty()) err = kj_last_error(); return; }
+            }
+        });
+        for (auto& x : workers) x.join();
+        if (!err.empty()) die(err);
+    }
     for (size_t k = 0; k < l1.size(); k++) {
         if (!table_fn.empty()) {     // kaiju2table's report from the per-taxon counts kept in HBM (one block of rows per data set, in list order)
             kj_table_opts to; memset(&to, 0, sizeof to); to.rank = table_rank.c_str();
