@@ -212,6 +212,10 @@ int kj_device_count(void);                        /* number of usable CUDA devic
  * block per warp, CRC-32 and length of every block checked there; only the compressed bytes cross to the device.  Should a later member of
  * such a file not be a BGZF block, zlib reads the rest from there.  Every other gzip file is inflated by zlib on one host thread per file.
  * A corrupt or truncated BGZF block is KJ_ERR_IO, and kj_last_error() names the file and the block's offset in it.
+ * in1 / in2 may name input that cannot seek -- a FIFO, a pipe, /dev/stdin or /dev/fd/N (bash's <(...)), a character device: it is read once,
+ * front to back, by one host thread, with the same result as the same bytes in a regular file (BGZF still inflated on the device).  A FIFO is
+ * opened without waiting for its writer, so one writer may open the two files of a pair in either order; a call that fails returns without
+ * waiting for a stalled writer.
  * `format` is one of the KJ_OUT_* line formats below (0 and 1 are the former `verbose` = 0 / 1).  Format 2 needs the KJ_STR_ACCESSION table,
  * formats 3 and 4 the KJ_STR_TAXON table and a context in params.name_mode (kj_set_output_strings); otherwise KJ_ERR_ARG before anything is
  * read.  With name_mode and input_is_protein the reader follows kaijup (kaijup.cpp:227-262): names are kept whole and the file type is the

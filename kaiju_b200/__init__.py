@@ -215,7 +215,7 @@ def classify_files_multi(classifiers, in1, in2=None, out_path=None, verbose=Fals
     """Classifier.classify_files over several Classifiers (same index and parameters; replicas or the members of create_group) in this
     process: one parser on the first one's GPU, whole batches classified by every Classifier, the output in input order and byte for byte
     what the first Classifier alone writes (kj_classify_files_multi).  Each Classifier counts the reads it classified (sum their counts()).
-    Returns (reads, classified lines) over all of them."""
+    in1 / in2 may be FIFOs, pipes or /dev/stdin as for Classifier.classify_files.  Returns (reads, classified lines) over all of them."""
     if fmt is None:
         fmt = OUT_KAIJU_IDS if verbose else OUT_KAIJU
     n = C.c_uint64(); k = C.c_uint64()
@@ -378,7 +378,8 @@ class Classifier:
     def classify_files(self, in1, in2=None, out_path=None, verbose=False, fmt=None):
         """FASTA/FASTQ(.gz) files -> kaiju output file, parsed / classified / formatted on the device (blocked gzip, BGZF, is inflated
         there too; other gzip by zlib on the host).  fmt: one of OUT_KAIJU (default), OUT_KAIJU_IDS (= verbose=True), OUT_KAIJU_V,
-        OUT_NAMES, OUT_NAMES_V (the last three need set_output_strings).  Returns (reads, classified lines)."""
+        OUT_NAMES, OUT_NAMES_V (the last three need set_output_strings).  in1 / in2 may also be FIFOs, pipes or /dev/stdin: read once, front
+        to back, with the output the same bytes give from a regular file.  Returns (reads, classified lines)."""
         if fmt is None:
             fmt = OUT_KAIJU_IDS if verbose else OUT_KAIJU
         n = C.c_uint64(); k = C.c_uint64()

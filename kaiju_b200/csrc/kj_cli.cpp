@@ -28,8 +28,8 @@ static bool g_pool = false;                            // -P: one index spread o
 static void die(const std::string& m) { fprintf(stderr, "Error: %s\n\n", m.c_str()); exit(EXIT_FAILURE); }
 static void usage(const char* prog) {
     fprintf(stderr, "kaiju-b200 (H100-native classification path of Kaiju)\n\nUsage:\n   %s -t nodes.dmp -f kaiju_db.fmi -i reads.fastq [-j reads2.fastq]\n\n"
-                    "Mandatory arguments:\n   -t FILENAME   Name of nodes.dmp file\n   -f FILENAME   Name of database (.fmi) file\n   -i FILENAME   Name of input file containing reads in FASTA or FASTQ format\n\n"
-                    "Optional arguments:\n   -j FILENAME   Name of second input file for paired-end reads\n   -o FILENAME   Name of output file. If not specified, output will be printed to STDOUT\n"
+                    "Mandatory arguments:\n   -t FILENAME   Name of nodes.dmp file\n   -f FILENAME   Name of database (.fmi) file\n   -i FILENAME   Name of input file containing reads in FASTA or FASTQ format (plain, gzip or BGZF;\n                 also a FIFO or pipe, e.g. /dev/stdin or <(zcat r1.fq.gz))\n\n"
+                    "Optional arguments:\n   -j FILENAME   Name of second input file for paired-end reads (may be a FIFO or pipe, as -i)\n   -o FILENAME   Name of output file. If not specified, output will be printed to STDOUT\n"
                     "   -z INT        accepted for compatibility (ignored: the GPU replaces the worker threads)\n   -a STRING     Run mode, either \"mem\"  or \"greedy\" (default: greedy)\n"
                     "   -e INT        Number of mismatches allowed in Greedy mode (default: 3)\n   -m INT        Minimum match length (default: 11)\n   -s INT        Minimum match score in Greedy mode (default: 65)\n"
                     "   -E FLOAT      Minimum E-value in Greedy mode (default: 0.01)\n   -x            Enable SEG low complexity filter (enabled by default)\n   -X            Disable SEG low complexity filter\n"

@@ -18,6 +18,7 @@
 // Included by kj_device.cu (one translation unit: it uses kj_ctx and launch()).
 #pragma once
 #include <fcntl.h>
+#include <sys/stat.h>
 #include <unistd.h>
 #include <zlib.h>
 #include <condition_variable>
@@ -25,6 +26,7 @@
 #include <mutex>
 #include <set>
 #include "kj_inflate.h"
+#include "kj_stream.h"
 #include "kj_format.h"
 
 // ------------------------------------------------------------------------------------------------
@@ -423,8 +425,25 @@ struct KjStaged { int slot = -1; size_t n = 0; bool eof = false; char last = 0; 
 // BGZF (a gzip file whose first member carries the "BC" extra subfield): the compressed bytes are read like a plain file's, the block chain is
 // walked on the host and the blocks are inflated on the device straight into the ring slot a plain chunk would have been copied to; a later
 // member that is no BGZF block sends the rest of the file to zlib.
+// Input that cannot seek (fstat: not a regular file -- a FIFO, a pipe, /dev/stdin, a character device) is read once, front to back, by the
+// reader thread alone (KjStream, kj_stream.h): its first 64 KiB are the format probe and then the start of the first chunk, BGZF round or zlib
+// input; a BGZF round carries what it did not consume to the front of the next round's buffer; other gzip goes through a z_stream.  The
+// descriptor is opened with O_NONBLOCK, so the two files of a pair are open before either has a writer, and every wait of the thread is a poll()
+// that halt() ends.
+// A pair of streams from one writer (samtools fastq -1 a -2 b): the parser fills side 0 up to its target (at most batch_max + chunk bytes of
+// text) before side 1, so file 2's reader must hold what the writer puts into file 2 meanwhile: its ring of `depth` = min(64, batch_max / chunk + 4)
+// chunks plus the chunk in its pinned buffer (and the pipe's own buffer).  That covers records of file 2 up to (depth + 1) * chunk /
+// (batch_max + chunk) times as long as file 1's -- 1.44 with the default 16 MB chunks and 128 MB batches, 3 with KJ_INGEST_CHUNK alone -- and, while
+// side 1 is filled, records of file 1 up to ((depth + 1) * chunk + batch_max) / (batch_max + chunk) times as long as file 2's (2.33, 3.5).  Mates
+// of 150 and 100 bases (about 1.47 : 1 in FASTQ bytes with short names) lie within both bounds with 150-base mates in file 1; a skew beyond them
+// stalls the writer and with it the call.
 struct KjFileReader {
     gzFile fp = nullptr; int fd = -1; uint64_t file_off = 0; std::string path; size_t chunk = 0; int device = 0; KjPinnedPool* pinned = nullptr;
+    bool is_stream = false; KjStream src; KjGzStream gz; size_t left_at = 0, left_n = 0;     // input that cannot seek; a BGZF round's unconsumed bytes
+    // Pairs: file 1's reader (follower = file 2's) hands its error to file 2's as lead_error.  The parser takes file 1's chunks before file 2's
+    // and ends only at the end of file 1, so that error ends the call whatever file 2 still holds; a wait for the next chunk of a file-2 stream
+    // returns it at once (the stream's writer may be waiting for file 1 to be read).
+    KjFileReader* follower = nullptr; std::string lead_error;
     char* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; bool pin_busy[2] = {false, false}; cudaStream_t stream = nullptr;
     std::vector<KjDevBuf> ring; std::vector<cudaEvent_t> ring_ev; std::deque<int> free_slots; std::deque<KjStaged> ready;
     std::mutex mu; std::condition_variable cv; std::thread th; bool stop = false;
@@ -458,16 +477,21 @@ struct KjFileReader {
     }
     int open(const std::string& p, size_t chunk_bytes, int depth, int device_, KjPinnedPool* pp) {
         path = p; chunk = chunk_bytes; device = device_; pinned = pp; stop = false; wstop = false; file_off = 0; inflated = 0; last_byte = 0; tm_read = tm_inflate = 0;
-        fd = ::open(p.c_str(), O_RDONLY);
-        if (fd < 0) { kj_err() = "Could not open file " + p; return KJ_ERR_IO; }
-        std::vector<uint8_t> head(65536); const ssize_t got = ::pread(fd, head.data(), head.size(), 0); const unsigned char* magic = head.data();
-        {   // BGZF is what the first member says it is: a gzip header with the "BC" subfield (its whole block lies within the first 64 KiB)
-            table.clear(); const int st = got > 0 ? kj_bgzf_walk(head.data(), (size_t)got, 0, 1, 0, 0, table).stop : KJ_BGZF_GARBAGE;
-            bgzf = !table.empty() || st == KJ_BGZF_PARTIAL;
+        left_at = left_n = 0;
+        fd = ::open(p.c_str(), O_RDONLY | O_NONBLOCK);           // a FIFO opens at once, with or without a writer
+        struct stat sb;
+        if (fd < 0 || fstat(fd, &sb) != 0) { if (fd >= 0) ::close(fd); fd = -1; kj_err() = "Could not open file " + p; return KJ_ERR_IO; }
+        is_stream = !S_ISREG(sb.st_mode);
+        if (is_stream) {      // the format is probed on the reader thread: the first read may wait for the writer
+            const int sfd = fd; fd = -1;
+            if (!src.open(sfd)) { src.close(); kj_err() = "Could not open file " + p + " (eventfd)"; return KJ_ERR_IO; }
+            return start(depth);
         }
-        rchunk = bgzf ? std::max<size_t>(chunk, 65536) : chunk; slot_bytes = rchunk + 16;
-        max_blocks = rchunk / 1024 + 64; tab_off = (rchunk + 63) & ~(size_t)63; st_off = tab_off + max_blocks * sizeof(KjBgzfBlock); last_off = st_off + max_blocks * 4; zbytes = last_off + 16;
-        if (!bgzf && got >= 2 && magic[0] == 0x1f && magic[1] == 0x8b) {             // other gzip: inflate through zlib; everything else is read as it is
+        (void)fcntl(fd, F_SETFL, fcntl(fd, F_GETFL) & ~O_NONBLOCK);
+        std::vector<uint8_t> head(65536); const ssize_t got = ::pread(fd, head.data(), head.size(), 0);
+        const int format = kj_input_format(head.data(), got > 0 ? (size_t)got : 0);
+        bgzf = format == KJ_INPUT_BGZF; layout();
+        if (format == KJ_INPUT_GZIP) {             // other gzip: inflate through zlib; everything else is read as it is
             ::close(fd); fd = -1; fp = gzopen(p.c_str(), "rb");
             if (!fp) { kj_err() = "Could not open file " + p; return KJ_ERR_IO; }
             gzbuffer(fp, 1 << 20);
@@ -478,10 +502,28 @@ struct KjFileReader {
             wgot.assign((rchunk + SLICE - 1) / SLICE, 0);
             for (unsigned t = 0; t < nt; t++) workers.emplace_back([this] { worker(); });
         }
+        return start(depth);
+    }
+    int start(int depth) {
         if ((int)ring.size() != depth) { ring.clear(); ring.resize((size_t)depth); }
         free_slots.clear(); ready.clear(); for (int k = 0; k < depth; k++) free_slots.push_back(k);
         th = std::thread([this] { run(); });
         return KJ_OK;
+    }
+    void layout() {        // the sizes of a round and of a ring slot, once the format is known
+        rchunk = bgzf ? std::max<size_t>(chunk, 65536) : chunk; slot_bytes = rchunk + 16;
+        max_blocks = rchunk / 1024 + 64; tab_off = (rchunk + 63) & ~(size_t)63; st_off = tab_off + max_blocks * sizeof(KjBgzfBlock); last_off = st_off + max_blocks * 4; zbytes = last_off + 16;
+    }
+    // a stream's first bytes (up to 64 KiB) decide its format as a file's do; they are put back in front of the stream.  false: the call is over
+    bool probe() {
+        std::vector<char> head(65536); size_t got = 0; bool eof = false;
+        const int r = src.fill(head.data(), head.size(), got, eof);
+        if (r) { if (r != KJ_STREAM_HALTED) fail("read error in file " + path); return false; }
+        const int format = kj_input_format((const uint8_t*)head.data(), got);
+        src.unread(head.data(), got);
+        bgzf = format == KJ_INPUT_BGZF; layout();
+        if (format == KJ_INPUT_GZIP && !gz.start()) { fail("Could not open file " + path + " (inflateInit2)"); return false; }
+        return true;
     }
     // one round of the worker pool: the rchunk bytes at file_off (fewer at the end of the file) into b.  false: read error
     bool read_round(char* b, size_t& got, bool& eof) {
@@ -511,8 +553,7 @@ struct KjFileReader {
             if (cudaEventSynchronize(f.ck.ev) != cudaSuccess) { fail("inflating " + path + " failed on the device"); return false; }
             tm_inflate += kj_ms_since(t0);
             const uint32_t* st = (const uint32_t*)(zpin[f.pb] + st_off); const KjBgzfBlock* tb = (const KjBgzfBlock*)(zpin[f.pb] + tab_off);
-            for (size_t i = 0; i < f.nblk; i++) if (st[i]) {
-                fail("corrupt BGZF block in file " + path + " at compressed offset " + std::to_string(f.off + tb[i].in_off - tb[i].hdr) + ": " + kj_inflate_strerror(st[i])); return false; }
+            for (size_t i = 0; i < f.nblk; i++) if (st[i]) { fail(kj_bgzf_block_error(path, f.off, tb[i], st[i])); return false; }
             if (f.ck.n) last_byte = zpin[f.pb][last_off];
             f.ck.last = last_byte; f.on = false;
             { std::lock_guard<std::mutex> lk(mu); ready.push_back(f.ck); }
@@ -526,16 +567,15 @@ struct KjFileReader {
             if (zdev[pb].grow(zbytes) != KJ_OK) { fail("cudaMalloc failed (compressed staging)"); return false; }
             char* b = zpin[pb]; size_t got = 0; bool ceof = false;
             auto t0 = std::chrono::steady_clock::now();
-            if (!read_round(b, got, ceof)) { fail("read error in file " + path); return false; }
+            if (is_stream) {         // the other buffer's unconsumed bytes (that round is in flight: its copy reads only the bytes it consumed), then the stream
+                const int r = kj_bgzf_top_up(src, b, rchunk, zpin[pb ^ 1], left_at, left_n, got, ceof);
+                if (r) { if (r != KJ_STREAM_HALTED) fail("read error in file " + path); return false; }
+            } else if (!read_round(b, got, ceof)) { fail("read error in file " + path); return false; }
             tm_read += kj_ms_since(t0);
-            table.clear();
-            const KjBgzfWalk w = kj_bgzf_walk((const uint8_t*)b, got, slot_bytes - 16, max_blocks, 0, 0, table);
-            bool eof = false, to_zlib = false;
-            if (w.stop == KJ_BGZF_END) eof = ceof;
-            else if (w.stop == KJ_BGZF_GARBAGE) eof = true;                  // zlib, too, ignores what follows the last member
-            else if (w.stop == KJ_BGZF_FOREIGN) to_zlib = true;
-            else if (w.stop == KJ_BGZF_BAD) { fail("corrupt BGZF header in file " + path + " at compressed offset " + std::to_string(file_off + w.consumed)); return false; }
-            else if (w.stop == KJ_BGZF_PARTIAL && (ceof || w.consumed == 0)) { fail("truncated BGZF block in file " + path + " at compressed offset " + std::to_string(file_off + w.consumed)); return false; }
+            const KjBgzfRound plan = kj_bgzf_plan((const uint8_t*)b, got, ceof, slot_bytes - 16, max_blocks, file_off, path, table);
+            if (!plan.error.empty()) { fail(plan.error); return false; }
+            const KjBgzfWalk w = plan.w; const bool eof = plan.eof, to_zlib = plan.to_zlib;
+            left_at = w.consumed; left_n = got - w.consumed;
             cur = Flight(); cur.pb = pb; cur.nblk = table.size(); cur.off = file_off; cur.on = true; cur.ck.n = (size_t)w.out_bytes; cur.ck.eof = eof;
             {   // a free staging buffer on the device
                 std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || !free_slots.empty(); }); if (stop) return false;
@@ -560,16 +600,25 @@ struct KjFileReader {
             prev = cur;
             if (!eof && !to_zlib) continue;
             if (!finish(prev) || eof) return false;
+            if (is_stream) {         // zlib takes the unconsumed bytes, then the rest of the stream
+                src.unread(b + left_at, left_n);
+                if (!gz.start()) { fail("Could not open file " + path + " (inflateInit2)"); return false; }
+                return true;
+            }
             if (::lseek(fd, (off_t)file_off, SEEK_SET) < 0 || !(fp = gzdopen(fd, "rb"))) { fail("Could not open file " + path); return false; }
             fd = -1; gzbuffer(fp, 1 << 20);
             return true;
         }
     }
-    void fail(const std::string& what) { KjStaged e; e.error = what; { std::lock_guard<std::mutex> lk(mu); ready.push_back(e); } cv.notify_all(); }
+    void fail(const std::string& what) {
+        KjStaged e; e.error = what; { std::lock_guard<std::mutex> lk(mu); ready.push_back(e); } cv.notify_all();
+        if (follower) { { std::lock_guard<std::mutex> lk(follower->mu); follower->lead_error = what; } follower->cv.notify_all(); }
+    }
     void run() {
         if (cudaSetDevice(device) != cudaSuccess) { fail("cudaSetDevice failed"); return; }
         if (!stream && cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) { fail("cudaStreamCreate failed"); return; }
         while (ring_ev.size() < ring.size()) { cudaEvent_t e; if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) { fail("cudaEventCreate failed"); return; } ring_ev.push_back(e); }
+        if (is_stream && !probe()) return;
         if (bgzf && !run_bgzf()) return;
         char prev_last = last_byte;
         for (uint64_t it = 0;; it++) {
@@ -583,6 +632,10 @@ struct KjFileReader {
             if (fd >= 0) {
                 if (!read_round(b, got, ck.eof)) ck.error = "read error in file " + path;
                 file_off += got;
+            } else if (is_stream) {
+                const int r = gz.on ? gz.read(src, b, chunk, got, ck.eof) : src.fill(b, chunk, got, ck.eof);
+                if (r == KJ_STREAM_HALTED) return;
+                if (r) ck.error = "read error in file " + path;
             } else while (got < chunk) {
                 const ssize_t r = (ssize_t)gzread(fp, b + got, (unsigned)std::min<size_t>(chunk - got, 1u << 30));
                 if (r < 0) { ck.error = "read error in file " + path; break; }
@@ -604,10 +657,16 @@ struct KjFileReader {
             if (last) return;
         }
     }
-    KjStaged next() { std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return !ready.empty(); }); KjStaged ck = ready.front(); ready.pop_front(); return ck; }
+    KjStaged next() {
+        std::unique_lock<std::mutex> lk(mu); cv.wait(lk, [&] { return stop || !ready.empty() || (is_stream && !lead_error.empty()); });
+        if (ready.empty()) { KjStaged e; e.error = stop ? "the call was stopped" : lead_error; return e; }      // halt(): the call is failing elsewhere
+        KjStaged ck = ready.front(); ready.pop_front(); return ck;
+    }
     void release_slot(int slot) { { std::lock_guard<std::mutex> lk(mu); free_slots.push_back(slot); } cv.notify_all(); }
+    // ends every wait of the reader thread and of next(), a read from a stream included
+    void halt() { { std::lock_guard<std::mutex> lk(mu); stop = true; } cv.notify_all(); src.halt(); }
     void close() {
-        { std::lock_guard<std::mutex> lk(mu); stop = true; } cv.notify_all();
+        halt();
         if (th.joinable()) th.join();
         { std::lock_guard<std::mutex> lk(wmu); wstop = true; } wcv.notify_all();
         for (auto& w : workers) if (w.joinable()) w.join();
@@ -617,6 +676,7 @@ struct KjFileReader {
         for (int k = 0; k < 2; k++) { if (zpin[k]) pinned->put(zpin[k], zbytes); zpin[k] = nullptr; }
         if (fp) gzclose(fp); fp = nullptr;
         if (fd >= 0) ::close(fd); fd = -1;
+        gz.end(); src.close(); is_stream = false;
         for (int k = 0; k < 2; k++) { if (pin[k]) pinned->put(pin[k], chunk); pin[k] = nullptr; pin_busy[k] = false; if (pin_ev[k]) cudaEventDestroy(pin_ev[k]); pin_ev[k] = nullptr; }
         ready.clear(); free_slots.clear(); wgen = 0; wslices = 0; wnext = 0; wleft = 0;
     }
@@ -719,6 +779,7 @@ struct KjFilesState {
     void reset_slots() { free_slot.clear(); for (int k = 0; k < KJ_FILE_SLOTS; k++) free_slot.push_back(k); }
     void end_call() {      // threads, files and in-flight copies of one call
         { std::lock_guard<std::mutex> lk(mu); abort = true; } cv.notify_all();
+        for (int f = 0; f < 2; f++) if (rd_open[f]) rd[f].halt();      // a parser waiting for a stream's next chunk returns too
         if (parser.joinable()) parser.join();
         for (int f = 0; f < 2; f++) {
             if (rd_open[f]) rd[f].close(); rd_open[f] = false;
@@ -1037,6 +1098,8 @@ static int kj_classify_files_impl(KjFilesRun& R, const char* in1, const char* in
     int rc;
     if (!S.sp) { int lo = 0, hi = 0; CK(cudaDeviceGetStreamPriorityRange(&lo, &hi)); CK(cudaStreamCreateWithPriority(&S.sp, cudaStreamNonBlocking, hi)); }    // the short parse kernels go first when SM slots free up
     const int depth = (int)std::min<size_t>(64, batch_max / chunk + 4);
+    for (int f = 0; f < 2; f++) S.rd[f].lead_error.clear();
+    S.rd[0].follower = paired ? &S.rd[1] : nullptr;
     for (int f = 0; f < S.nfiles; f++) { if ((rc = S.rd[f].open(fn[f], chunk, depth, c->device, &S.pinned))) return rc; S.rd_open[f] = true; }
     // output buffers: two per lane of every context, one more for the oldest batch (KjWriter)
     if ((rc = S.wr.open(out_path, R.out_cap, 1 + 2 * R.n_ctx, &S.pinned))) return rc; S.wr_open = true;
