@@ -16,6 +16,7 @@
 #include <cstring>
 #include <atomic>
 #include <mutex>
+#include <stdexcept>
 #include <string>
 #include <thread>
 #include <vector>
@@ -26,6 +27,11 @@ static uint32_t g_max_read_len = KJ_MAX_READ_LEN;      // -L: longest mate admit
 static uint64_t g_host_bytes = 0;                      // -H: pinned host memory the index may take when it does not fit in HBM (kj_create_tiered)
 static bool g_pool = false;                            // -P: one index spread over the HBM of the -d devices (kj_create_group)
 static void die(const std::string& m) { fprintf(stderr, "Error: %s\n\n", m.c_str()); exit(EXIT_FAILURE); }
+// -l, -s, -m and -e are read as the reference reads them (std::stoi, kaiju.cpp:110-166): the leading number of the argument, which must fit
+// in an int.  An argument without one, or out of range, is reported and the option keeps its value.
+static bool read_int(const char* s, int& v) {
+    try { v = std::stoi(s); return true; } catch (const std::exception&) { return false; }
+}
 static void usage(const char* prog) {
     fprintf(stderr, "kaiju-b200 (H100-native classification path of Kaiju)\n\nUsage:\n   %s -t nodes.dmp -f kaiju_db.fmi -i reads.fastq [-j reads2.fastq]\n\n"
                     "Mandatory arguments:\n   -t FILENAME   Name of nodes.dmp file\n   -f FILENAME   Name of database (.fmi) file\n   -i FILENAME   Name of input file containing reads in FASTA or FASTQ format (plain, gzip or BGZF;\n                 also a FIFO or pipe, e.g. /dev/stdin or <(zcat r1.fq.gz))\n\n"
@@ -60,10 +66,10 @@ int main(int argc, char** argv) {
             case 't': nodes_fn = optarg; break;
             case 'i': in1 = optarg; break;
             case 'j': in2 = optarg; break;
-            case 'l': { int v = atoi(optarg); if (v < 7) { die("Seed length must be >= 7."); } P.seed_length = (uint32_t)v; break; }
-            case 's': { int v = atoi(optarg); if (v <= 0) die("Min Score (-s) must be greater than 0."); P.min_score = (uint32_t)v; break; }
-            case 'm': { int v = atoi(optarg); if (v <= 0) die("Min fragment length (-m) must be greater than 0."); P.min_fragment_length = (uint32_t)v; break; }
-            case 'e': { int v = atoi(optarg); if (v < 0) die("Number of mismatches must be >= 0."); P.mismatches = (uint32_t)v; break; }
+            case 'l': { int v; if (!read_int(optarg, v)) { fprintf(stderr, "Invalid argument in -l %s\n", optarg); break; } if (v < 7) die("Seed length must be >= 7."); P.seed_length = (uint32_t)v; break; }
+            case 's': { int v; if (!read_int(optarg, v)) { fprintf(stderr, "Invalid argument in -s %s\n", optarg); break; } if (v <= 0) die("Min Score (-s) must be greater than 0."); P.min_score = (uint32_t)v; break; }
+            case 'm': { int v; if (!read_int(optarg, v)) { fprintf(stderr, "Invalid argument in -m %s\n", optarg); break; } if (v <= 0) die("Min fragment length (-m) must be greater than 0."); P.min_fragment_length = (uint32_t)v; break; }
+            case 'e': { int v; if (!read_int(optarg, v)) { fprintf(stderr, "Invalid numerical argument in -e %s\n", optarg); break; } if (v < 0) die("Number of mismatches must be >= 0."); P.mismatches = (uint32_t)v; break; }
             case 'E': { P.min_evalue = atof(optarg); if (P.min_evalue <= 0.0) die("E-value threshold must be greater than 0."); break; }
             case 'z': { if (atoi(optarg) <= 0) die("Number of threads (-z) must be greater than 0."); break; }
             case 'n': break;

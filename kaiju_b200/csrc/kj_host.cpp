@@ -175,6 +175,8 @@ int kj_check_params(const kj_params& p) {
     if (p.mode == 0 && p.use_evalue) { kj_err() = "E-value calculation is only possible in Greedy mode"; return KJ_ERR_ARG; }   // kaiju.cpp:202
     if (p.mode == 1 && p.mismatches > KJ_MAX_MM) { kj_err() = "more than 8 mismatches (-e) are not supported"; return KJ_ERR_UNSUPPORTED; }
     if (p.mode == 1 && (p.min_score == 0 || p.seed_length == 0)) { kj_err() = "min_score and seed_length must be > 0"; return KJ_ERR_ARG; }
+    // the reference reads -l and -s into an int (kaiju.cpp:112-138), and the Greedy kernels compare both as int (kj_core_greedy.h)
+    if (p.seed_length > (uint32_t)INT32_MAX || p.min_score > (uint32_t)INT32_MAX) { kj_err() = "seed_length and min_score must be at most 2^31 - 1"; return KJ_ERR_ARG; }
     if (p.use_evalue && !(p.min_evalue > 0.0)) { kj_err() = "E-value threshold must be greater than 0"; return KJ_ERR_ARG; }
     return KJ_OK;
 }
